@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """bench.py — view-frames/sec of the V3D denoising hot path (EulerEDMSampler -> VideoUNet -> VideoDecoder).
 
-    python bench.py --gpus N --steps K --warmup W            # B200-native arm (this repo's kernels)
+    python bench.py --gpus N --steps K --warmup W            # native arm (this repo's H100 kernels)
+    python bench.py ... --dump-outputs DIR                   # also write the last timed step's frames to DIR/*.npy
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path (oracle port) on host cores
 
 One "step" = the whole hot path for one image: T=18 views, 512x512 (latent 4x64x64), 25 Euler-EDM steps with CFG
@@ -13,7 +14,7 @@ Timed regions (CUDA events on the launching stream, barrier + synchronize on bot
   value : inputs already resident in HBM
   e2e   : through the public API with pinned HOST buffers, H2D of noise+conditioning and D2H of the uint8 frames
           inside the timed region.
-`roofline` describes the dominant kernel family (the tcgen05 GEMM / implicit conv kernel): algorithmic FLOPs of its
+`roofline` describes the dominant kernel family (the wgmma GEMM / implicit conv kernel): algorithmic FLOPs of its
 launches in one step / their summed CUDA-event durations, against MEASURED_PEAKS.json.
 """
 from __future__ import annotations
@@ -33,7 +34,8 @@ sys.path.insert(0, str(ROOT))
 # algorithmic FLOPs of the reference modules (BASELINE.md §2; FlopCounterMode on the reference, 2*MAC, CFG-batched)
 F_UNET_TF = {14: 35.542, 18: 45.677, 24: 60.884, 25: 63.419}
 F_DEC_TF = {14: 42.599, 18: 54.771, 24: 73.028, 25: 76.070}
-FALLBACK_PEAKS = {"bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "hbm_gbs": 6650.0}
+# without MEASURED_PEAKS.json: NVIDIA's H100 SXM data sheet (dense BF16, HBM3 at a 700 W limit), not measured rates
+FALLBACK_PEAKS = {"bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "hbm_gbs": 3350.0}
 
 
 def work_tf(T: int, S: int, latent: int) -> float:
@@ -80,7 +82,7 @@ def load_traffic():
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks/throttle reasons sampled DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -370,7 +372,7 @@ def workload_config(args, where: str) -> dict:
             "parallelism": (f"one image over {args.gpus} ranks, plan '{args.shard}' (views: frame blocks with K|V "
                             "all-gather, conv halos, 3-D GN all-reduce; cfg: the CFG halves on a rank pair)"
                             if getattr(args, "shard", "images") != "images" else f"image-dp{args.gpus}"),
-            "l2_policy": "working set per step (3 GB bf16 weights + activations) exceeds the 126 MB L2; no explicit flush",
+            "l2_policy": "working set per step (3 GB bf16 weights + activations) exceeds the 50 MB L2; no explicit flush",
             "weights": "random-init (per-name seeded, oracle/synth.py), zero-init modules re-randomised"}
 
 
@@ -428,7 +430,7 @@ def assemble_line(args, *, world, secs, secs_e2e, launches, clocks, h2d_bytes, d
         "gpu_launches": launches,
         "clocks": clocks,
         "roofline": {
-            "bound": "tensor", "kernel": "gemm_tc_kernel (tcgen05 GEMM / temporal conv / implicit 3x3 conv)",
+            "bound": "tensor", "kernel": "gemm_tc_kernel (wgmma GEMM / temporal conv / implicit 3x3 conv)",
             "achieved": achieved, "peak": peak_tf,
             "unit": "TFLOP/s", "frac": achieved / peak_tf if achieved is not None else None,
             # DRAM bytes (read + write) of ONE launch of the dominant kernel at its top-level shape - the implicit 3x3
@@ -447,7 +449,7 @@ def assemble_line(args, *, world, secs, secs_e2e, launches, clocks, h2d_bytes, d
             "gemm_shapes_decode": shape_table(decode_shapes)[:20],
             "hbm_bound_families": dict(hbm_rows, peak_gbs=peaks_hbm,
                                        note="algorithmic bytes (each tensor read / written once) over summed CUDA-event "
-                                            "durations of one eager step; many of these tensors fit the 126 MB L2"),
+                                            "durations of one eager step; many of these tensors fit the 50 MB L2"),
             "model": {"reference_accounting_tflop_per_step": model_tf,
                       "achieved_tflops": model_tf / (secs / args.steps), "frac": model_tf / (secs / args.steps) / peak_tf},
         },
@@ -503,16 +505,19 @@ def parity_check(eng, dev, manifest) -> dict:
     with torch.no_grad():
         out = eng.model.diffusion_model(xin, gold["timesteps"].to(dev), ctx, y, None, T,
                                         torch.zeros(2, T, device=dev))
+    out = out[:, :, ::gold["out_stride"], ::gold["out_stride"]]    # the fixture keeps every out_stride-th pixel
     res = {"unet_forward": {"rel_l2": rel(out, gold["out"]), "cosine": cos(out, gold["out"]),
                             "finite": bool(torch.isfinite(out).all()), "fixture": "tests/golden/unet_v3d512.pt"}}
     md = manifest["decoder_v3d512"]
     gold = torch.load(gold_dir / "decoder_v3d512.pt")
     with torch.no_grad():
-        img = eng.first_stage_model.decoder(gold["z"].to(dev) / 0.18215, timesteps=md["T"])
+        z = torch.randn(md["B"], 4, md["latent_hw"], md["latent_hw"], generator=torch.Generator().manual_seed(gold["z_seed"]))
+        img = eng.first_stage_model.decoder(z.to(dev) / 0.18215, timesteps=md["T"])
     st = gold["stride"]
+    y0, y1, x0, x1 = gold["crop"]
     res["decode"] = {"rel_l2": rel(img[:, :, ::st, ::st], gold["out_sub"]),
                      "cosine": cos(img[:, :, ::st, ::st], gold["out_sub"]),
-                     "rel_l2_full_frames": rel(img[gold["full_frames"]], gold["out_full"]),
+                     "rel_l2_full_res_window": rel(img[gold["full_frames"]][:, :, y0:y1, x0:x1], gold["out_full"]),
                      "finite": bool(torch.isfinite(img).all()), "fixture": "tests/golden/decoder_v3d512.pt"}
     res["tolerance"] = dict(PARITY_TOL)
     res["against"] = "outputs of the real reference modules (fp32, CPU) on the same seeded weights and inputs"
@@ -664,6 +669,31 @@ def measure_strong(args, eng, dev, rank, world, T, L) -> dict:
     return out
 
 
+DUMP_CAP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir: str, frames) -> None:
+    """Write what the timed path returned in its last step, the uint8 THWC frames a caller receives, as float32 .npy,
+    so that two builds run with the same arguments (same seeded inputs and weights) can be compared output for output.
+    Up to 64 MB (18 x 512 x 512 x 3 frames are 54 MB) the whole array goes to DIR/frames.npy; beyond that a fixed,
+    seeded sample of image rows goes to DIR/frames_rows.npy [k, W, 3] with their flat indices t * H + h (float64) in
+    DIR/frames_row_index.npy."""
+    import numpy as np
+    import torch
+
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    f = frames.detach().float().cpu()
+    if f.numel() * 4 <= DUMP_CAP_BYTES:
+        np.save(d / "frames.npy", f.numpy())
+        return
+    rows = f.reshape(-1, f.shape[-2], f.shape[-1])                 # [T * H, W, 3]
+    k = DUMP_CAP_BYTES // (rows[0].numel() * 4 + 8)
+    idx = torch.randperm(rows.shape[0], generator=torch.Generator().manual_seed(0))[:k].sort().values
+    np.save(d / "frames_rows.npy", rows[idx].numpy())
+    np.save(d / "frames_row_index.npy", idx.double().numpy())
+
+
 def run_native(args) -> None:
     import torch
 
@@ -764,14 +794,15 @@ def run_native(args) -> None:
         l0 = ops.launch_count() + eng.model.diffusion_model.replayed_launches
         w0 = time.time()
         ev0.record()
+        out = None
         for _ in range(k):
-            fn()
+            out = fn()
         ev1.record()
         torch.cuda.synchronize()
         w1 = time.time()
         parallel.barrier()
         secs = parallel.max_over_ranks(ev0.elapsed_time(ev1) / 1000.0, dev)
-        return secs, ops.launch_count() + eng.model.diffusion_model.replayed_launches - l0, (w0, w1)
+        return secs, ops.launch_count() + eng.model.diffusion_model.replayed_launches - l0, (w0, w1), out
 
     for _ in range(args.warmup):
         step_resident()
@@ -781,11 +812,16 @@ def run_native(args) -> None:
     if rank == 0:
         clocks.start()
         time.sleep(0.3)
-    secs, launches, (w0, w1) = timed(step_resident, args.steps)
+    secs, launches, (w0, w1), last = timed(step_resident, args.steps)
     clk = clocks.stop(w0, w1) if rank == 0 else None
+    if args.dump_outputs:
+        # the view-sharded plans return this rank's frame block: a caller receives the gathered image
+        frames = plan.gather_frames(last) if plan is not None else last
+        if rank == 0:
+            dump_outputs(args.dump_outputs, frames)
 
     step_e2e()  # warm the e2e-only pieces (pinned copies)
-    secs_e2e, _, _ = timed(step_e2e, args.steps)
+    secs_e2e, _, _, _ = timed(step_e2e, args.steps)
 
     # ---- roofline of the dominant kernel family + per-family breakdown: every launch of ONE step is bracketed
     #      by CUDA events on the launching stream (a separate pass, so the timed region above carries no probes)
@@ -923,11 +959,16 @@ def main():
     ap.add_argument("--no-strong", action="store_true",
                     help="N > 1, image-parallel run: skip the one-image-over-N-GPUs sub-measurement (`strong`)")
     ap.add_argument("--no-parity", action="store_true", help="skip the pre-timing parity check against tests/golden")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's output (the uint8 frames a caller receives, "
+                         "as float32) to DIR/frames.npy, or a seeded row sample of it beyond 64 MB")
     ap.add_argument("--shard", choices=["images", "views", "cfg", "cfg+views"], default="images",
                     help="images (default): one image per GPU, weak scaling.  ONE image over the GPUs (strong scaling): "
                          "views = frame blocks (K|V all-gather, conv halos, 3-D GroupNorm all-reduce); cfg = the [uc; c] "
                          "halves on 2 GPUs (one all-gather per network evaluation); cfg+views = both (>= 4 GPUs)")
     args = ap.parse_args()
+    if args.dump_outputs and args.steps < 1:
+        ap.error("--dump-outputs writes the output of the last timed step: it needs --steps >= 1")
     if args.warmup < 3 and args.impl == "native":
         print("warning: timing rules ask for >= 3 warm-up steps", file=sys.stderr)
     if args.impl == "reference":

@@ -1,5 +1,5 @@
 /*
- * v3d_b200 — C ABI of the B200 (sm_100a) kernels behind V3D's denoising hot path.
+ * v3d_b200 — C ABI of the H100 (sm_90a) kernels behind V3D's denoising hot path.
  *
  * The reference (heheyas/V3D) has no FFI of its own: every GPU op on the path is a PyTorch library
  * call.  Each entry point below therefore names the reference call site(s) it replaces
@@ -38,7 +38,7 @@ const char* v3d_last_error(void);
 int64_t v3d_launch_count(void);
 
 /* ------------------------------------------------------------------------------------------
- * Tensor-core GEMM family (tcgen05.mma, TMEM accumulators, TMA-staged operands).
+ * Tensor-core GEMM family (wgmma, register accumulators, TMA-staged operands).
  *
  *   D[row, n] = s0 * act( sum_k A[row, k] * B[n, k] + bias[n] + fbias[row / rows_per_frame, n] )
  *               + s1 * R1[row, n] + s2 * R2[row, n]
@@ -151,8 +151,8 @@ int v3d_softmax_rows_f32(const void* x, void* y, int64_t rows, int32_t n, float 
  * (row stride ld_qkv elements); heads are 64-column groups.
  * ------------------------------------------------------------------------------------------ */
 /* F.scaled_dot_product_attention / xformers FMHA, attention.py:337-341,432-444: per (sample, head)
- * softmax(q k^T scale) v over ntok tokens; token rows are sample-major. tcgen05 MMAs (S = QK^T and O = PV with
- * TMEM accumulators), TMA-staged Q/K/V tiles, warp-specialised fp32 softmax. */
+ * softmax(q k^T scale) v over ntok tokens; token rows are sample-major. wgmma MMAs (S = QK^T and O = PV with
+ * register accumulators), TMA-staged Q/K/V tiles, fp32 online softmax. */
 int v3d_attention_spatial(const void* q, const void* k, const void* v, void* o, int64_t ld_qkv, int64_t ld_o,
                           int32_t nbatch, int32_t ntok, int32_t nheads, float scale, void* stream);
 /* validation twin of v3d_attention_spatial on mma.sync (same contract); not used by the product path. */

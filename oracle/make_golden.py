@@ -34,7 +34,7 @@ def _pin(name: str, ref: torch.Tensor, ora: torch.Tensor) -> float:
 
 
 def _unet_case(ns, tag: str, model_channels: int, T: int, hw: int, wseed: int, sigma: float, manifest: dict,
-               tap_stride: int = 1):
+               tap_stride: int = 1, out_stride: int = 1):
     kw = dict(reference_shim.V3D_UNET_KW)
     kw["model_channels"] = model_channels
     net = ns.video_model.VideoUNet(**kw).eval()
@@ -67,7 +67,10 @@ def _unet_case(ns, tag: str, model_channels: int, T: int, hw: int, wseed: int, s
     err = _pin(tag, ref, ora)
     for w in want:
         _pin(f"{tag}:{w}", taps_ref[w], taps_or[w])
-    blob = {"out": ref, "timesteps": ts}
+    # out_stride > 1 (the BASELINE-size fixture): every out_stride-th pixel of the output, so the file stays under 1 MB
+    blob = {"out": ref[:, :, ::out_stride, ::out_stride].contiguous(), "timesteps": ts}
+    if out_stride > 1:
+        blob["out_stride"] = out_stride
     for w in want:
         # keep fixtures small: frames {0 (uc half), T (c half)}, every 8th channel, fp16
         # (tap_stride > 1: also every tap_stride-th pixel -- the BASELINE-size fixture)
@@ -75,7 +78,8 @@ def _unet_case(ns, tag: str, model_channels: int, T: int, hw: int, wseed: int, s
     torch.save(blob, OUT / f"{tag}.pt")
     manifest[tag] = dict(kind="unet_forward", model_channels=model_channels, T=T, latent_hw=hw, weight_seed=wseed,
                          input_seed=23, sigma=sigma, pin_err=err, ref_cpu_seconds=round(t_ref, 2),
-                         out_std=ref.std().item(), tap_stride=tap_stride)
+                         out_std=ref.std().item(), tap_stride=tap_stride,
+                         **({"out_stride": out_stride} if out_stride > 1 else {}))
     return net, sd, spec
 
 
@@ -138,7 +142,7 @@ def _sampler_variant_case(ns, net, sd, spec, tag: str, T: int, hw: int, num_step
 
 
 def _decoder_case(ns, tag: str, ch: int, T: int, B: int, hw: int, wseed: int, manifest: dict, z=None,
-                  full_frames=None, stride: int = 1):
+                  full_frames=None, stride: int = 1, crop=None):
     kw = dict(reference_shim.V3D_DECODER_KW)
     kw["ch"] = ch
     dec = ns.temporal_ae.VideoDecoder(**kw).eval()
@@ -161,13 +165,17 @@ def _decoder_case(ns, tag: str, ch: int, T: int, B: int, hw: int, wseed: int, ma
     if full_frames is None:
         torch.save({"out": ref, "z": z}, OUT / f"{tag}.pt")
     else:
-        # BASELINE-size fixture: `full_frames` complete frames + every stride-th pixel of all frames, fp16
-        # (the decoder output is an image in about [-1.5, 1.5]: fp16 rounding 5e-4 relative, far below the tolerance)
-        torch.save({"z": z, "full_frames": list(full_frames), "out_full": ref[list(full_frames)].half(),
-                    "stride": stride, "out_sub": ref[:, :, ::stride, ::stride].half()}, OUT / f"{tag}.pt")
+        # BASELINE-size fixture (under 1 MB): the full-resolution window `crop` = (y0, y1, x0, x1) of the `full_frames`
+        # + every stride-th pixel of all frames, fp16 (the decoder output is an image in about [-1.5, 1.5]: fp16
+        # rounding 5e-4 relative, far below the tolerance); z is the seeded draw above, regenerated from z_seed
+        y0, y1, x0, x1 = crop
+        torch.save({"z_seed": 77, "full_frames": list(full_frames), "crop": list(crop),
+                    "out_full": ref[list(full_frames)][:, :, y0:y1, x0:x1].half().contiguous(),
+                    "stride": stride, "out_sub": ref[:, :, ::stride, ::stride].half().contiguous()}, OUT / f"{tag}.pt")
     manifest[tag] = dict(kind="decode", ch=ch, T=T, B=B, latent_hw=hw, weight_seed=wseed, z_seed=77, pin_err=err,
                          ref_cpu_seconds=round(t_ref, 2), out_std=ref.std().item(),
-                         full_frames=list(full_frames) if full_frames is not None else None, stride=stride)
+                         full_frames=list(full_frames) if full_frames is not None else None, stride=stride,
+                         **({"crop": list(crop)} if crop is not None else {}))
 
 
 def _encoder_case(ns, tag: str, ch: int, B: int, hw: int, wseed: int, manifest: dict):
@@ -292,7 +300,8 @@ def main(argv):
         _edm_step_case(ns, net, sd, spec, "edm_full_step", T=4, hw=32, num_steps=1, manifest=manifest)
     if want("unet_v3d512"):
         # BASELINE.json configs[1] network evaluation: full width, T=18, latent 64x64, CFG batch 36 (one forward)
-        _unet_case(ns, "unet_v3d512", 320, T=18, hw=64, wseed=3, sigma=3.0, manifest=manifest, tap_stride=4)
+        _unet_case(ns, "unet_v3d512", 320, T=18, hw=64, wseed=3, sigma=3.0, manifest=manifest, tap_stride=4,
+                   out_stride=2)
     if want("edm_v3d512_25step"):
         # 25 accumulating Euler-EDM steps (CFG, T=18) on the full-width network at the smallest latent that
         # exercises every level (16x16 -> 2x2 at the bottom)
@@ -301,7 +310,7 @@ def main(argv):
     if want("decoder_v3d512"):
         # BASELINE.json configs[1] decode: 18 frames, latent 64x64 -> 512x512, one chunk
         _decoder_case(ns, "decoder_v3d512", 128, T=18, B=18, hw=64, wseed=6, manifest=manifest,
-                      full_frames=(0, 11), stride=4)
+                      full_frames=(0, 11), stride=8, crop=(128, 320, 128, 320))
     if want("decoder_small"):
         _decoder_case(ns, "decoder_small", 64, T=3, B=3, hw=16, wseed=4, manifest=manifest)
     if want("decoder_small_2videos"):

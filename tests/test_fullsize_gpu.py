@@ -3,7 +3,7 @@ decode to 512 x 512), where the oracle is far too slow to be the checker:
 
   * the implicit 3x3 convolution (TMA gather, 9 taps) equals the explicit im2row + linear GEMM path on the same input -
     two independent operand-gather implementations of one contraction, same K order;
-  * the tcgen05 flash attention equals its mma.sync twin at N = 4096 keys;
+  * the wgmma flash attention equals its mma.sync twin at N = 4096 keys;
   * the halo'd-operand temporal conv over 8 uneven frame blocks equals the dense temporal conv, bit for bit;
   * a CFG-batched UNet forward (B = 36 = [uc; c]) equals two B = 18 forwards of its halves (nothing may leak between
     the two videos of a batch; exercises 32-bit row / offset arithmetic at the largest shapes);
@@ -67,7 +67,7 @@ def test_flash_attention_equals_mma_twin_full_size():
     ops.attention_spatial_mma(qkv, b, n, ntok, heads, 0.125)
     torch.cuda.synchronize()
     r = _rel(a, b)
-    print("tcgen05 vs mma.sync attention at N=4096: rel-L2", r)
+    print("wgmma vs mma.sync attention at N=4096: rel-L2", r)
     assert r <= 1e-2                                   # two softmax formulations; bf16 P and output
 
 

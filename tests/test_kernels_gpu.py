@@ -53,7 +53,7 @@ def assert_close(got, ref, rtol=1.0 / 128, atol=2e-2, what=""):
 
 
 # --------------------------------------------------------------------------------------------
-# tcgen05 GEMM: linear mode
+# tensor-core (wgmma) GEMM: linear mode
 # --------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("M,K,N", [
     (128, 64, 16), (128, 64, 64), (128, 128, 128), (256, 320, 320), (384, 1280, 1280),
@@ -103,10 +103,9 @@ def test_gemm_epilogue_full():
 @pytest.mark.parametrize("N", [320, 256, 128, 64])
 @pytest.mark.parametrize("inplace", [False, True])
 def test_gemm_single_residual_many_tiles(N, inplace):
-    """bf16 output + one residual over far more tiles than SMs (every CTA walks several tiles; N = 320 gives an odd
-    number of 32-column sub-tiles, so the two epilogue groups swap shares from tile to tile), residual separate or in
-    place (out is r1, the transformer's `t = t + f(t)` pattern), row tail included.  Also the case the opt-in epilogue
-    variants (CTA pairs, TMA-staged residual) are re-run on."""
+    """bf16 output + one residual over far more tiles than SMs (every CTA walks several tiles and reuses its staging
+    buffer once the previous tile's TMA stores have read it; N = 320 gives an odd number of 32-column sub-tiles), residual
+    separate or in place (out is r1, the transformer's `t = t + f(t)` pattern), row tail included."""
     M, K = 128 * 500 + 40, 64
     a, w = rnd(M, K), rnd(N, K, scale=K ** -0.5)
     bias = torch.randn(N, device=DEV)
@@ -323,6 +322,7 @@ def test_softmax_rows():
 # --------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("nb,ntok,heads", [(2, 16, 4), (3, 64, 20), (2, 256, 10), (2, 1024, 5), (1, 4096, 5),
                                            (2, 200, 2), (1, 1000, 3), (2, 300, 2), (1, 600, 1), (3, 2048, 2)])
+# "tcgen05" names the product kernel (v3d_attention_spatial, now wgmma); the id is kept so the test's history stays one
 @pytest.mark.parametrize("impl", ["tcgen05", "mma"])
 def test_attention_spatial(nb, ntok, heads, impl):
     c = heads * 64
@@ -473,10 +473,6 @@ def test_sampler_arithmetic_and_u8():
     assert (u8.int() - ref.int()).abs().max() <= 1  # fp rounding of the *255 product may differ by one ulp
 
 
-# ---- kernel variants that the default path selects per shape (V3D_GEMM_2CTA / V3D_GEMM_RTMA "auto"): the child processes
-# below force them onto EVERY eligible launch of the GEMM / conv tests of this file
-
-
 def test_heun_step_kernel():
     """v3d_heun_step vs the formula of HeunEDMSampler.possible_correction_step (sampling.py:221-237)."""
     n, per = 6, 4 * 16 * 16
@@ -493,31 +489,6 @@ def test_heun_step_kernel():
     d2 = (xe - den2) / sn.clamp_min(1e-30)[:, None]
     ref = torch.where(sn[:, None] > 0, x + (d + d2) / 2 * dt, x + dt * d)
     assert torch.allclose(out, ref, rtol=1e-5, atol=1e-5)
-
-
-def test_gemm_cta_pair_path_subprocess():
-    """The cta_group::2 (CTA pair) GEMM tiles (V3D_GEMM_2CTA, read once per process; default "auto" = per shape):
-    re-run the GEMM / conv tests of this file in a child process with the tiles forced on, under a hard timeout."""
-    import subprocess
-    import sys
-
-    env = dict(os.environ, V3D_GEMM_2CTA="1")
-    res = subprocess.run([sys.executable, "-m", "pytest", __file__, "-x", "-q", "-m", "gpu", "-k",
-                          "(gemm or conv3x3 or temporal_conv) and not subprocess"], env=env, capture_output=True, text=True, timeout=600)
-    assert res.returncode == 0, res.stdout[-3000:] + res.stderr[-2000:]
-
-
-def test_gemm_tma_staged_residual_subprocess():
-    """EPI_BF16RT (V3D_GEMM_RTMA=1, read once per process): the single residual of a bf16-output GEMM / conv arrives as
-    128 x 32 TMA sub-tiles two sub-tiles ahead instead of per-lane global loads.  The GEMM / conv / temporal-conv tests
-    of this file (several carry R1, some in place) re-run in a child with the switch on, under a hard timeout."""
-    import subprocess
-    import sys
-
-    env = dict(os.environ, V3D_GEMM_RTMA="1")
-    res = subprocess.run([sys.executable, "-m", "pytest", __file__, "-x", "-q", "-m", "gpu", "-k",
-                          "(gemm or conv3x3 or temporal_conv) and not subprocess"], env=env, capture_output=True, text=True, timeout=600)
-    assert res.returncode == 0, res.stdout[-3000:] + res.stderr[-2000:]
 
 
 @pytest.mark.parametrize("poly", [2])

@@ -1,21 +1,21 @@
-"""Boundary proof with the REFERENCE's own plugin machinery (SURVEY.md 8(b); VERDICT r1 item 9).
+"""Boundary proof against the REFERENCE's engine layout (SURVEY.md 8(b); VERDICT r1 item 9).
 
-The reference's `DiffusionEngine.__init__` (sgm/models/video_diffusion.py:35-105) is run - unmodified, imported in place
-from /root/reference through oracle/reference_shim.py - on a config whose hot-path `target:` strings are the drop-ins of
-INTEGRATION.md section A.  `instantiate_from_config` / `get_obj_from_str` (sgm/util.py:170-187) therefore resolve and
-construct the v3d_b200 classes exactly as `scripts/pub/V3D_512.py:72-112` would.  Checked:
+The reference's `DiffusionEngine.__init__` (sgm/models/video_diffusion.py:35-105), run unmodified on the reduced-width
+V3D_512 config below with its own `target:` strings, builds an engine whose `state_dict()` key -> shape map is stored,
+as a sha256 digest with its entry counts, in tests/golden/reference_engine_state_dict.json (written by
+oracle/make_golden_state_dict.py from the reference checkout).
+The drop-in engine built from the drop-in targets of INTEGRATION.md section A is checked against it:
 
-  * the engine the reference builds from the drop-in targets has the SAME `state_dict()` keys and shapes as the engine it
-    builds from its own targets (network, first-stage decoder; the conditioner is the reference's unconditional stub);
-  * `load_state_dict(strict=True)` of the reference-built engine's weights into the drop-in-built engine;
-  * the reference's `init_from_ckpt` (video_diffusion.py:123-168, safetensors branch) loads a checkpoint written from the
-    reference-built engine into the drop-in-built engine with no missing / unexpected keys;
-  * the drop-in `v3d_b200.sgm.models.video_diffusion.DiffusionEngine` accepts the same checkpoint.
+  * the SAME `state_dict()` keys and shapes (network, first-stage decoder, everything else);
+  * `load_state_dict(strict=True)` of a checkpoint with the reference's layout, and the weights round-trip;
+  * `init_from_ckpt` (the safetensors branch of video_diffusion.py:123-168) loads such a checkpoint with no missing /
+    unexpected keys.
 
-CPU only (construction and weight plumbing; no kernels run).  Skipped where /root/reference is absent (the GPU box).
+CPU only (construction and weight plumbing; no kernels run).
 """
 import copy
-import importlib
+import hashlib
+import json
 import sys
 from pathlib import Path
 
@@ -25,10 +25,7 @@ import torch
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
 
-from oracle import reference_shim  # noqa: E402
-
-pytestmark = pytest.mark.skipif(not reference_shim.available(), reason="/root/reference not present")
-
+GOLDEN = ROOT / "tests" / "golden" / "reference_engine_state_dict.json"
 WIDTH, DEC_CH, T = 64, 64, 4
 
 
@@ -52,7 +49,8 @@ def _config(prefix: str, first_stage_prefix: str):
             "target": first_stage_prefix + ".models.autoencoder.AutoencodingEngine",
             "params": {
                 "loss_config": {"target": "torch.nn.Identity"},
-                "regularizer_config": {"target": "sgm.modules.autoencoding.regularizers.DiagonalGaussianRegularizer"},
+                "regularizer_config": {"target": first_stage_prefix + ".modules.autoencoding.regularizers."
+                                                 "DiagonalGaussianRegularizer"},
                 "encoder_config": {"target": "torch.nn.Identity"},
                 "decoder_config": {"target": prefix + ".modules.autoencoding.temporal_ae.VideoDecoder",
                                    "params": dict(attn_type="vanilla", double_z=True, z_channels=4, resolution=256,
@@ -68,56 +66,65 @@ def _config(prefix: str, first_stage_prefix: str):
     )
 
 
-@pytest.fixture(scope="module")
-def ref_engine_cls():
-    reference_shim.install()
-    reference_shim._stub("kornia")
-    reference_shim._stub("open_clip")
-    mods = sys.modules["sgm.modules"]
-    enc = importlib.import_module("sgm.modules.encoders.modules")
-    # what sgm/modules/__init__.py:1-6 defines (the package __init__ itself is bypassed by the shim: it pulls CLIP)
-    mods.GeneralConditioner = enc.GeneralConditioner
-    mods.UNCONDITIONAL_CONFIG = {"target": "sgm.modules.GeneralConditioner", "params": {"emb_models": []}}
-    vd = importlib.import_module("sgm.models.video_diffusion")
-    return vd.DiffusionEngine
+def layout_digest(layout) -> str:
+    """sha256 over the sorted `key:shape` lines of a state-dict layout."""
+    lines = "\n".join(f"{k}:{','.join(str(int(d)) for d in shape)}" for k, shape in sorted(layout.items()))
+    return hashlib.sha256(lines.encode()).hexdigest()
 
 
 @pytest.fixture(scope="module")
-def engines(ref_engine_cls):
+def golden():
+    return json.loads(GOLDEN.read_text())
+
+
+@pytest.fixture(scope="module")
+def drop():
+    from v3d_b200.sgm.models.video_diffusion import DiffusionEngine
+
     torch.manual_seed(0)
-    ref = ref_engine_cls(**copy.deepcopy(_config("sgm", "sgm")))
-    drop = ref_engine_cls(**copy.deepcopy(_config("v3d_b200.sgm", "v3d_b200.sgm")))
-    return ref, drop
+    return DiffusionEngine(**copy.deepcopy(_config("v3d_b200.sgm", "v3d_b200.sgm")))
+
+
+@pytest.fixture(scope="module")
+def layout(drop, golden):
+    """The drop-in engine's layout, once it is shown to be the reference's."""
+    mine = {k: tuple(v.shape) for k, v in drop.state_dict().items()}
+    assert len(mine) == golden["entries"] and layout_digest(mine) == golden["sha256"]
+    return mine
 
 
 def _hot_path_items(sd):
-    return {k: tuple(v.shape) for k, v in sd.items()
+    return {k: tuple(v) for k, v in sd.items()
             if k.startswith("model.diffusion_model.") or k.startswith("first_stage_model.decoder.")}
 
 
-def test_reference_loader_builds_dropins_with_identical_state_dict(engines):
-    ref, drop = engines
+def _reference_shaped_weights(layout):
+    """Seeded values in the reference's layout (a stand-in for a checkpoint the reference engine would write)."""
+    g = torch.Generator().manual_seed(0)
+    return {k: torch.randn(shape, generator=g) if shape else torch.randn((), generator=g) for k, shape in sorted(layout.items())}
+
+
+def test_reference_loader_builds_dropins_with_identical_state_dict(drop, golden):
     import v3d_b200.decoder
     import v3d_b200.sampling
     import v3d_b200.unet
 
-    # the reference's instantiate_from_config constructed OUR classes
+    # the drop-in targets constructed OUR classes
     assert isinstance(drop.model.diffusion_model, v3d_b200.unet.VideoUNet)
     assert isinstance(drop.first_stage_model.decoder, v3d_b200.decoder.VideoDecoder)
     assert isinstance(drop.sampler, v3d_b200.sampling.EulerEDMSampler)
     assert isinstance(drop.denoiser, v3d_b200.sampling.Denoiser)
-    assert type(drop.model).__module__ == "sgm.modules.diffusionmodules.wrappers"     # the reference's own wrapper
-    a, b = _hot_path_items(ref.state_dict()), _hot_path_items(drop.state_dict())
-    assert len(a) > 1000 and a == b
+    mine = {k: tuple(v.shape) for k, v in drop.state_dict().items()}
+    hot = _hot_path_items(mine)
+    # the network and the first-stage decoder have the reference's keys and shapes
+    assert len(hot) > 1000 and len(hot) == golden["hot_path_entries"]
+    assert layout_digest(hot) == golden["hot_path_sha256"]
     # nothing else differs either (conditioner stub has no weights; the denoiser / sampler hold no parameters)
-    extra_ref = set(ref.state_dict()) - set(a)
-    extra_drop = set(drop.state_dict()) - set(b)
-    assert extra_ref == extra_drop, (sorted(extra_ref ^ extra_drop)[:10])
+    assert len(mine) == golden["entries"] and layout_digest(mine) == golden["sha256"]
 
 
-def test_strict_load_state_dict_round_trip(engines):
-    ref, drop = engines
-    sd = {k: v.clone() for k, v in ref.state_dict().items()}
+def test_strict_load_state_dict_round_trip(drop, layout):
+    sd = {k: v.reshape(layout[k]) for k, v in _reference_shaped_weights(layout).items()}
     missing, unexpected = drop.load_state_dict(sd, strict=True)
     assert not missing and not unexpected
     back = drop.state_dict()
@@ -126,23 +133,15 @@ def test_strict_load_state_dict_round_trip(engines):
         assert torch.equal(back[k], sd[k]), k
 
 
-def test_reference_init_from_ckpt_loads_into_dropins(engines, ref_engine_cls, tmp_path):
+def test_reference_init_from_ckpt_loads_into_dropins(layout, tmp_path):
     from safetensors.torch import save_file
 
-    ref, drop = engines
+    from v3d_b200.sgm.models.video_diffusion import DiffusionEngine
+
+    want = {k: v.reshape(layout[k]).contiguous() for k, v in _reference_shaped_weights(layout).items()}
     path = str(tmp_path / "v3d_small.safetensors")
-    save_file({k: v.contiguous() for k, v in ref.state_dict().items()}, path)
-    # 1) the REFERENCE engine class, drop-in targets, the reference's own checkpoint loader
-    cfg = copy.deepcopy(_config("v3d_b200.sgm", "v3d_b200.sgm"))
-    eng = ref_engine_cls(ckpt_path=path, **cfg)
-    want = ref.state_dict()
+    save_file(want, path)
+    eng = DiffusionEngine(ckpt_path=path, **copy.deepcopy(_config("v3d_b200.sgm", "v3d_b200.sgm")))
     got = eng.state_dict()
     for k, v in want.items():
         assert torch.equal(got[k], v), k
-    # 2) the drop-in engine class on the same checkpoint and config
-    from v3d_b200.sgm.models.video_diffusion import DiffusionEngine
-
-    eng2 = DiffusionEngine(ckpt_path=path, **copy.deepcopy(cfg))
-    got2 = eng2.state_dict()
-    for k in _hot_path_items(want):
-        assert torch.equal(got2[k], want[k]), k

@@ -129,7 +129,7 @@ def test_gemm_kv_scatter_equals_output_columns(M, K, C):
     """Fused projection GEMM -> all-gather: the epilogue stores the K|V columns (>= C of the packed q|k|v output) a second
     time into every destination matrix - here two local buffers, one with a wider row stride; across GPUs the same
     stores go to IPC-mapped peer memory.  The copies must be bit-identical to the output columns, the output itself
-    unchanged, rows past M untouched (one-CTA and, at M >= 8192, CTA-pair tiles)."""
+    unchanged, rows past M untouched."""
     from v3d_b200 import ops
 
     g = torch.Generator(device=DEV).manual_seed(M + C)
@@ -241,12 +241,12 @@ def test_view_sharded_engine_peer_transport_one_gpu():
     _run_engine_pair("gloo", one_gpu=True, transport="peer")
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs")
 def test_view_sharded_engine_matches_unsharded_nccl():
     _run_engine_pair("nccl", one_gpu=False)                       # default transport over NCCL groups: peer memory
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs")
 def test_view_sharded_engine_matches_unsharded_nccl_collectives():
     _run_engine_pair("nccl", one_gpu=False, transport="nccl")    # torch.distributed collectives on the data path
 
@@ -322,17 +322,17 @@ def test_cfg_split_engine_peer_transport_one_gpu():
     _run_plan("cfg", 2, "gloo", one_gpu=True, transport="peer")
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 4, reason="needs four GPUs (gpurun --gpus 4): four processes that "
+@pytest.mark.skipif(torch.cuda.device_count() < 4, reason="needs four GPUs: four processes that "
                     "spin-wait on each other's signals do not make progress under the time-slicing of ONE GPU")
 def test_cfg_views_engine_peer_transport():
     _run_plan("cfg+views", 4, "nccl", one_gpu=False, transport="peer")
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs")
 def test_cfg_split_engine_matches_unsharded_nccl():
     _run_plan("cfg", 2, "nccl", one_gpu=False)
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 4, reason="needs four GPUs (gpurun --gpus 4)")
+@pytest.mark.skipif(torch.cuda.device_count() < 4, reason="needs four GPUs")
 def test_cfg_views_engine_matches_unsharded_nccl():
     _run_plan("cfg+views", 4, "nccl", one_gpu=False)

@@ -1,7 +1,7 @@
-"""Spatial attention with PEAKED score rows: the tcgen05 kernel keeps a lagged softmax reference and rescales its
-TMEM-resident output rows only when a key tile overshoots it by more than 2^8 (csrc/attention_tc.cu).  Random unit-scale
-inputs (test_kernels_gpu.py) never take that branch; here the key magnitude grows along the sequence, so the row
-maximum jumps by far more than 2^8 between tiles and the rescale path runs many times.  Checker: fp32 ATen SDPA on the
+"""Spatial attention with PEAKED score rows: the wgmma kernel keeps a running row maximum and rescales its
+register-resident output rows and running sum whenever a key tile raises it (csrc/attention_tc.cu).  Here the key
+magnitude grows (or shrinks) along the sequence, so the row maximum jumps by far more than 2^8 between tiles and the
+rescale path runs with large factors many times.  Checker: fp32 ATen SDPA on the
 same bf16-rounded inputs.  (File name sorts last: this case was added after the round-1 GPU budget was spent.)
 """
 import pytest
@@ -38,8 +38,8 @@ def test_attention_spatial_peaked_rows(nb, ntok, heads, order):
     rel = ((got - ref).norm() / ref.norm()).item()
     assert torch.isfinite(got).all(), "non-finite attention output"
     assert rel <= 2e-2, f"peaked-row attention rel-L2 {rel:.4f}"
-    # same inputs through the mma.sync twin (exact running max, no lagged reference): the two kernels must agree
+    # same inputs through the mma.sync twin (an independent online-softmax implementation): the two kernels must agree
     out2 = torch.empty_like(out)
     ops.attention_spatial_mma(qkv, out2, nb, ntok, heads, 64 ** -0.5)
     rel2 = ((got - out2.float()).norm() / ref.norm()).item()
-    assert rel2 <= 2e-2, f"tcgen05 vs mma.sync rel-L2 {rel2:.4f}"
+    assert rel2 <= 2e-2, f"wgmma vs mma.sync rel-L2 {rel2:.4f}"

@@ -9,8 +9,6 @@
 #     gpurun --gpus 4 --timeout 900  -- 'NGPU=4 bash tools/gpu_round.sh nccl_tests strongN'
 # Stages:
 #   tests         the GPU suite (pytest -m gpu)
-#   pair / rtma   the GEMM / conv tests with the CTA-pair (V3D_GEMM_2CTA=1) or TMA-staged-residual (V3D_GEMM_RTMA=1) tiles
-#                 forced on, then the per-shape microbenchmark with the switch off / on
 #   attn_poly     FMA-pipe exp2 variants of the spatial attention (V3D_ATTN_POLY=1..3): tests, then timings 0..3
 #   micro_all     tools/microbench.py: every kernel family at its V3D_512 shapes
 #   bench         bench.py (default N=1) -> gpurun_out/bench.json
@@ -39,19 +37,6 @@ for stage in "$@"; do
   case "$stage" in
     tests)
       run 1500 tests_gpu.log $PY -m pytest tests -m gpu -x -q ;;
-    pair)
-      # the staged bring-up probe first: bounded waits, names the primitive that misbehaves instead of hanging
-      [ -x tools/ubench/pair_min ] || nvcc -gencode arch=compute_100a,code=sm_100a -std=c++17 --expt-relaxed-constexpr \
-        -I include -I v3d_b200/csrc -o tools/ubench/pair_min tools/ubench/pair_min.cu v3d_b200/csrc/host_util.cu
-      run 60 pair_probe.log tools/ubench/pair_min
-      run 300 pair_tests.log $PY -m pytest tests/test_kernels_gpu.py -m gpu -q -x -k "cta_pair"
-      run 300 micro_single.log $PY tools/microbench.py gemm conv
-      V3D_GEMM_2CTA=1 run 300 micro_pair.log $PY tools/microbench.py gemm conv ;;
-    rtma)
-      # TMA-staged residual epilogue (V3D_GEMM_RTMA=1): tests under a timeout (a barrier-phase mistake would hang),
-      # then the per-shape microbenchmark with the switch off / on (the +R1 rows are the ones that should move)
-      run 400 rtma_tests.log $PY -m pytest tests/test_kernels_gpu.py -m gpu -q -x -k "tma_staged_residual"
-      V3D_GEMM_RTMA=1 run 300 micro_rtma.log $PY tools/microbench.py gemm conv ;;
     attn_poly)
       run 600 attn_poly_tests.log $PY -m pytest tests/test_kernels_gpu.py -m gpu -q -k "attention_poly_exp2"
       for k in 0 1 2 3; do V3D_ATTN_POLY=$k run 300 "micro_attn_poly$k.log" $PY tools/microbench.py attn; done ;;
@@ -61,8 +46,6 @@ for stage in "$@"; do
       run 900 bench_ref.json $PY bench.py --impl reference --steps 2 --warmup 1 ;;
     sweep)
       run 1500 sweep.log $PY tools/sweep.py ;;
-    bench_pair)
-      V3D_GEMM_2CTA=1 run 900 bench_pair.json $PY bench.py --steps 3 --warmup 3 --no-cpu-baseline ;;
     ncu_launches)
       V3D_CUDA_GRAPH=0 run 1200 ncu_launches.log ncu --metrics gpu__time_duration.sum --clock-control none -c 9000 --csv \
         --log-file gpurun_out/launches.csv $PY bench.py --steps 1 --warmup 0 --edm-steps 1 --no-cpu-baseline --no-parity ;;

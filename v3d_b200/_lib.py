@@ -106,7 +106,7 @@ def load():
         return _lib
     if not _LIB_PATH.exists():
         raise V3DLibraryError(
-            f"{_LIB_PATH} is missing: the sm_100a kernels were not built. "
+            f"{_LIB_PATH} is missing: the sm_90a kernels were not built. "
             "Run `python -m v3d_b200.build` (needs nvcc); there is no CPU fallback for the product path."
         )
     lib = C.CDLL(str(_LIB_PATH))

@@ -1,7 +1,7 @@
-"""In-tree build of libv3d_b200.so (sm_100a only) with plain nvcc; no torch, no CMake.
+"""In-tree build of libv3d_b200.so (sm_90a, H100) with plain nvcc; no torch, no CMake.
 
 `python -m v3d_b200.build` compiles every csrc/*.cu that changed into build/obj and links
-v3d_b200/_lib/libv3d_b200.so.  The .so is git-ignored but ships with gpurun snapshots.
+v3d_b200/_lib/libv3d_b200.so.  Both are build products and stay out of git.
 """
 from __future__ import annotations
 
@@ -21,19 +21,16 @@ OBJ_DIR = REPO / "build" / "obj"
 LIB_DIR = ROOT / "_lib"
 LIB_PATH = LIB_DIR / "libv3d_b200.so"
 
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    *ARCH,
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
-    # nvcc starts compressing the embedded cubin once it passes ~10 MB (the GEMM family does since the opt-in epilogue
-    # variants were added); keep the fat binary uncompressed, like every build that has run on the hardware so far
+    # keep the embedded cubin uncompressed (nvcc compresses large fat binaries by default): no decompression at load
     "--no-compress",
     "-I", str(INCLUDE), "-I", str(CSRC),
 ]
-# V3D_GEMM_DIAG=1 builds the GEMM with its diagnostics (role timelines, stage-skipping switches) compiled in
-if os.environ.get("V3D_GEMM_DIAG"):
-    NVCC_FLAGS.append("-DV3D_GEMM_DIAG")
 
 
 def _nvcc() -> str:
@@ -84,7 +81,7 @@ def build(verbose: bool = False, force: bool = False) -> Path:
         objs = list(ex.map(lambda s: _compile_one(nvcc, s, verbose), srcs))
     newest = max(o.stat().st_mtime for o in objs)
     if force or not LIB_PATH.exists() or LIB_PATH.stat().st_mtime < newest:
-        cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC", "--no-compress",
+        cmd = [nvcc, "-shared", *ARCH, "-Xcompiler", "-fPIC", "--no-compress",
                "-o", str(LIB_PATH), *map(str, objs)]
         res = subprocess.run(cmd, capture_output=True, text=True)
         if res.returncode != 0:

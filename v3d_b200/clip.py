@@ -8,7 +8,7 @@ tensors); the state_dict here has the same keys - `model.visual.*` (the ViT) and
 `model.{positional_embedding, text_projection, logit_scale, token_embedding.weight, ln_final.*}`, which are loaded and
 never used - so `clip_model.load_state_dict(clip_sd)` of V3D_512.py:148-152 works unchanged.
 
-Runs once per image, so the schedule favours reuse over speed: every contraction is the tcgen05 GEMM of the denoiser
+Runs once per image, so the schedule favours reuse over speed: every contraction is the wgmma GEMM of the denoiser
 (`v3d_gemm_bf16`), LayerNorm and softmax are the path's kernels, and torch is used for layout glue only (patch
 unfolding, the class token / positional add, head-major repacking, the bicubic resize of the preprocessing):
   * conv1 (14 x 14 stride-14 patches, no bias) = unfold + GEMM with K = 588 zero-padded to 640;

@@ -4,7 +4,7 @@
 247-262.  Runs once per image; the only arithmetic is the sinusoidal embedding (`v3d_timestep_embedding`).
 
 Oracle pinned bit-exactly against the real GeneralConditioner (tests/golden/conditioning.pt); host logic tested on CPU,
-the device path in tests/test_kernels_gpu.py::test_concat_timestep_embedder_device (green on B200).
+the device path in tests/test_kernels_gpu.py::test_concat_timestep_embedder_device.
 """
 from __future__ import annotations
 

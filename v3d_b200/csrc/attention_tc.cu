@@ -1,47 +1,40 @@
-// Spatial self-attention on the 5th-gen tensor cores (head dim 64, bf16 operands, fp32 softmax).
+// Spatial self-attention on the Hopper tensor cores (wgmma; head dim 64, bf16 operands, fp32 softmax).
 //
 // One CTA = one (sample, head) x 128 queries; it streams 64-key K/V tiles:
-//   warp 0      : TMA producer (Q once; K_j, V_j through a 3-stage mbarrier ring, 128B swizzle)
-//   warp 1      : TMEM allocator + single-thread tcgen05.mma issuer
-//                   S_j = Q K_j^T   (128x64x64, A,B K-major)                       -> TMEM S[j&1] (2 x 64 columns)
-//                   O  += P_j V_j   (128x64x64, A = P K-major in smem, B = V MN-major) -> TMEM O (64 columns)
-//                 S_{j+1} is issued BEFORE P_j V_j, so the next scores are ready when the softmax warps come back.
-//   warps 2..5  : softmax: thread r owns query row r = its TMEM lane.  The 64 scores of the tile are pulled into
-//                 registers once (the S buffer is released immediately), row max, exp2, row sum, bf16 P into the
-//                 swizzled smem operand tile P[j&1].
-// O stays in TMEM for the whole key loop.  The softmax runs against a lagged row maximum: the reference point only
-// moves when the tile maximum exceeds it by more than 2^8 (then the warp rescales its O rows in TMEM and the running
-// sum); otherwise P is simply up to 256x larger, which fp32 sums and bf16 P hold without loss.  Mathematically the
-// result is the exact softmax; only rounding differs.
-// TMEM per CTA: 256 columns; shared memory ~97 KB -> two CTAs per SM.
+//   warp 8      : TMA producer (Q once; K_j, V_j through a 3-stage mbarrier ring, 128B swizzle)
+//   warps 0..7  : two consumer warpgroups, 64 query rows each:
+//                   S_j = Q K_j^T   wgmma m64n64k16 x 4, A = Q and B = K_j K-major in shared memory -> registers
+//                   online softmax on the register fragment (a row lives in the four lanes of a quad)
+//                   O  += P_j V_j   wgmma m64n64k16 x 4, A = P straight from registers (the S fragment re-packed as
+//                                   bf16), B = V_j MN-major in shared memory
+// O and the running max / sum stay in registers for the whole key loop; when the row maximum grows, O and the sum are
+// rescaled in place.  Shared memory ~65 KB, so several CTAs share an SM and one CTA's softmax overlaps another's MMAs.
 #include <cstdlib>
 #include <type_traits>
 
 #include "common.cuh"
 #include "host_util.cuh"
 #include "v3d_b200.h"
+#include "wgmma.cuh"
 
 namespace v3d {
 
 constexpr int AT_BM = 128;
 constexpr int AT_BN = 64;
-constexpr int AT_THREADS = 192;
+constexpr int AT_THREADS = 288;
 constexpr int AT_KVSTAGES = 3;
-constexpr int AT_QTILE = 128 * 128;                // bytes of a [128][64] bf16 tile (Q, P)
+constexpr int AT_QTILE = 128 * 128;                // bytes of a [128][64] bf16 tile (Q)
 constexpr int AT_KTILE = 64 * 128;                 // bytes of a [64][64] bf16 tile (K, V)
 constexpr int AT_OFF_Q = 0;
 constexpr int AT_OFF_K = AT_OFF_Q + AT_QTILE;
 constexpr int AT_OFF_V = AT_OFF_K + AT_KVSTAGES * AT_KTILE;
-constexpr int AT_OFF_P = AT_OFF_V + AT_KVSTAGES * AT_KTILE;  // 2 buffers
-constexpr int AT_OFF_BAR = AT_OFF_P + 2 * AT_QTILE;
-constexpr int AT_SMEM = AT_OFF_BAR + 256;
-constexpr uint32_t AT_TMEM_COLS = 256;
-constexpr float AT_RESCALE_LOG2 = 8.0f;            // move the softmax reference only for a > 2^8 overshoot
+constexpr int AT_OFF_BAR = AT_OFF_V + AT_KVSTAGES * AT_KTILE;
+constexpr int AT_SMEM = AT_OFF_BAR + 256 + 1024;   // + slack to align the base to 1024 B
 
 // 2^x for a pair of fp32 values on the FMA pipe (no MUFU): round-to-nearest split x = n + f with the 1.5 * 2^23 magic
 // add, degree-3 minimax polynomial for 2^f on [-0.5, 0.5] (max relative error 8.0e-5, a 25th of a bf16 half-ulp), then
 // n is added into the exponent field (the integer sits in the low mantissa bits of the magic sum, so `bits << 23` is
-// n << 23).  x must be >= -126 (callers clamp); large positive x does not occur (lagged reference: x <= 8 + noise).
+// n << 23).  x is clamped to >= -126; x <= 0 here (scores minus the running row maximum).
 __device__ __forceinline__ void exp2_poly2(float x0, float x1, float& p0, float& p1) {
   const uint64_t magic = pack2(12582912.0f, 12582912.0f);
   const uint64_t x2 = pack2(fmaxf(x0, -126.0f), fmaxf(x1, -126.0f));
@@ -59,24 +52,20 @@ __device__ __forceinline__ void exp2_poly2(float x0, float x1, float& p0, float&
 }
 
 // POLY: how many of the 8 key chunks of a tile take their exp2 from exp2_poly2 instead of MUFU ex2.approx
-// (0 = none, the validated kernel; 1 = every 4th chunk, 2 = every 2nd, 3 = three of four).  The softmax is
-// MUFU-bound (16 ex2 / clk / SM against 128 fp32 lanes): moving part of the row to the FMA pipe balances the two.
+// (0 = none, the default; 1 = every 4th chunk, 2 = every 2nd, 3 = three of four): moves part of the softmax's
+// exponentials from the MUFU pipe to the FMA pipe.
 template <int POLY>
 __global__ void __launch_bounds__(AT_THREADS, 2)
 attn_tc_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
                const __grid_constant__ CUtensorMap mapV, bf16* __restrict__ O, long long ldo, int ntok,
                float scale_log2e) {
-  extern __shared__ __align__(1024) uint8_t at_smem[];
-  uint8_t* smem = at_smem;
+  extern __shared__ uint8_t at_smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(at_smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + AT_OFF_BAR);
   uint64_t* q_full = bars + 0;
   uint64_t* kv_full = bars + 1;    // [3]
-  uint64_t* kv_empty = bars + 4;   // [3]
-  uint64_t* s_full = bars + 7;     // [2]
-  uint64_t* s_empty = bars + 9;    // [2]  128 arrivals: every softmax thread has its scores in registers
-  uint64_t* p_ready = bars + 11;   // [2]  128 arrivals
-  uint64_t* pv_done = bars + 13;   // [2]  P_j V_j retired (P[j&1] reusable, O readable)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 15);
+  uint64_t* kv_empty = bars + 4;   // [3]  one arrival per consumer warpgroup
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * AT_BM;
@@ -85,35 +74,19 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__
   const int nkv = (ntok + AT_BN - 1) / AT_BN;
 
   if (threadIdx.x == 0) {
-    if (smem_u32(smem) & 1023u) __trap();  // the swizzled operand tiles need a 1024-byte aligned base
     tma_prefetch_desc(&mapQ);
     tma_prefetch_desc(&mapK);
     tma_prefetch_desc(&mapV);
     mbar_init(q_full, 1);
     for (int i = 0; i < AT_KVSTAGES; ++i) {
       mbar_init(&kv_full[i], 1);
-      mbar_init(&kv_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&s_full[i], 1);
-      mbar_init(&s_empty[i], 128);
-      mbar_init(&p_ready[i], 128);
-      mbar_init(&pv_done[i], 1);
+      mbar_init(&kv_empty[i], 2);
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, AT_TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tS = tmem_base;            // 2 x 64 columns
-  const uint32_t tO = tmem_base + 128;      // 64 columns
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       mbar_arrive_expect_tx(q_full, AT_QTILE);
       tma_load_3d(smem + AT_OFF_Q, &mapQ, q_full, head * 64, q0, b);
@@ -130,479 +103,120 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = umma_idesc_bf16(128, 64, 0, 0);
-      constexpr uint32_t idesc_pv = umma_idesc_bf16(128, 64, 0, 1);  // B (= V) is MN-major: d contiguous
-      const uint64_t dq = umma_desc_k_sw128(smem_u32(smem + AT_OFF_Q));
-      auto issue_s = [&](int j, int st) {
-        const uint64_t dk = umma_desc_k_sw128(smem_u32(smem + AT_OFF_K + st * AT_KTILE));
-        const uint32_t d_s = tS + static_cast<uint32_t>((j & 1) * 64);
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          tc_mma_f16(d_s, dq + static_cast<uint64_t>(2 * k), dk + static_cast<uint64_t>(2 * k), idesc_s, k != 0);
-        tc_commit(&s_full[j & 1]);
-      };
-      mbar_wait(q_full, 0);
-      mbar_wait(&kv_full[0], 0);
-      tc_fence_after();
-      issue_s(0, 0);
-      int st = 0;       // ring stage of tile j
-      uint32_t ph = 0;  // its phase
-      for (int j = 0; j < nkv; ++j) {
-        int st1 = st + 1;
-        uint32_t ph1 = ph;
-        if (st1 == AT_KVSTAGES) {
-          st1 = 0;
-          ph1 ^= 1u;
-        }
-        if (j + 1 < nkv) {
-          mbar_wait(&kv_full[st1], ph1);
-          mbar_wait(&s_empty[(j + 1) & 1], (((j + 1) >> 1) & 1) ^ 1u);  // softmax j-1 holds its scores in registers
-          tc_fence_after();
-          issue_s(j + 1, st1);
-        }
-        mbar_wait(&p_ready[j & 1], (j >> 1) & 1);
-        tc_fence_after();
-        const uint32_t vbase = smem_u32(smem + AT_OFF_V + st * AT_KTILE);
-        const uint64_t dp0 = umma_desc_k_sw128(smem_u32(smem + AT_OFF_P + (j & 1) * AT_QTILE));
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          const uint64_t dv = umma_desc_mn_sw128(vbase + kk * 2048, AT_KTILE);
-          tc_mma_f16(tO, dp0 + static_cast<uint64_t>(2 * kk), dv, idesc_pv, (j | kk) != 0);
-        }
-        tc_commit(&pv_done[j & 1]);
-        tc_commit(&kv_empty[st]);
-        st = st1;
-        ph = ph1;
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    const int r = q * 32 + lane;
-    const uint32_t lane_base = static_cast<uint32_t>(q * 32) << 16;
-    const int sw = r & 7;
-    float m_ref = -INFINITY, l_run = 0.f;
-    const uint64_t sl2 = pack2(scale_log2e, scale_log2e);
+    return;
+  }
 
-    // One 64-key tile. TAIL = the tile crosses ntok: keys beyond it are masked (only the last tile can be one).
-    auto softmax_tile = [&](int j, auto tail_tag) {
-      constexpr bool TAIL = decltype(tail_tag)::value;
-      const int kbase = j * AT_BN;
-      const int sb = j & 1;
-      uint32_t s[64];
-      tmem_ld32p(tS + lane_base + static_cast<uint32_t>(sb * 64), s);
-      tmem_ld32p(tS + lane_base + static_cast<uint32_t>(sb * 64 + 32), s + 32);
-      tmem_ld_wait();
-      tc_fence_before();
-      mbar_arrive(&s_empty[sb]);  // the scores live in registers now: S[sb] may take tile j+2
-      // ---- row max (FMNMX3: two elements per instruction)
+  // ---- consumers.  Fragment of a 64 x 64 fp32 wgmma result: x[4 c + 2 h + e] = row 16 wi + lane / 4 + 8 h of the
+  // warpgroup's 64, column 8 c + 2 (lane % 4) + e.
+  const int cw = warp >> 2;
+  const int wi = warp & 3;
+  const int cq = (lane & 3) * 2;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  const uint64_t dq = gmma_desc_k_sw128(smem_u32(smem + AT_OFF_Q + cw * 64 * 128));
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  mbar_wait(q_full, 0);
+
+  auto key_tile = [&](int j, int st, auto tail_tag) {
+    constexpr bool TAIL = decltype(tail_tag)::value;
+    const int kbase = j * AT_BN;
+    float s[32];
+    const uint64_t dk = gmma_desc_k_sw128(smem_u32(smem + AT_OFF_K + st * AT_KTILE));
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      Wgmma<64>::ss(s, dq + static_cast<uint64_t>(2 * k), dk + static_cast<uint64_t>(2 * k), k != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    if (TAIL) {
+#pragma unroll
+      for (int c = 0; c < 8; ++c)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (kbase + 8 * c + cq + e >= ntok) s[4 * c + e] = s[4 * c + 2 + e] = -INFINITY;
+    }
+    float msc[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
       float mx = -INFINITY;
 #pragma unroll
-      for (int i = 0; i < 64; i += 2) {
-        float a0 = __uint_as_float(s[i]), a1 = __uint_as_float(s[i + 1]);
-        if (TAIL) {
-          if (kbase + i >= ntok) a0 = -INFINITY;
-          if (kbase + i + 1 >= ntok) a1 = -INFINITY;
-        }
-        mx = fmaxf(fmaxf(a0, a1), mx);
-      }
-      if (j == 0) {
-        m_ref = mx;  // nothing accumulated yet
-      } else {
-        const bool need = (mx - m_ref) * scale_log2e > AT_RESCALE_LOG2;
-        if (__any_sync(0xffffffffu, need)) {
-          // move the reference for the rows that overshot: O rows and the running sum shrink by 2^(old - new)
-          float fac = 1.0f;
-          if (need) {
-            fac = ex2_approx((m_ref - mx) * scale_log2e);
-            m_ref = mx;
-          }
-          l_run *= fac;
-          mbar_wait(&pv_done[(j - 1) & 1], ((j - 1) >> 1) & 1);  // O holds tiles 0..j-1
-          tc_fence_after();
+      for (int c = 0; c < 8; ++c) mx = fmaxf(mx, fmaxf(s[4 * c + 2 * h], s[4 * c + 2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      // every key tile holds at least one key < ntok, so mx is finite
+      if (mx > m_run[h]) {
+        const float fac = ex2_approx((m_run[h] - mx) * scale_log2e);  // 0 on the first tile
+        m_run[h] = mx;
+        l_run[h] *= fac;
 #pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            uint32_t o[16];
-            tmem_ld16p(tO + lane_base + static_cast<uint32_t>(c * 16), o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * fac);
-            tmem_st16p(tO + lane_base + static_cast<uint32_t>(c * 16), o);
-          }
-          tmem_st_wait();
+        for (int c = 0; c < 8; ++c) {
+          o[4 * c + 2 * h] *= fac;
+          o[4 * c + 2 * h + 1] *= fac;
         }
       }
-      // P[sb] was last read by P_{j-2} V_{j-2}
-      if (j >= 2) mbar_wait(&pv_done[sb], ((j - 2) >> 1) & 1);
-      // ---- P = exp2(s*scale - m_ref*scale), row sum, bf16 P into the swizzled smem A-operand tile
-      const float msc = m_ref * scale_log2e;
-      const uint64_t nm2 = pack2(-msc, -msc);
-      uint64_t lsum = 0ull;
-      uint8_t* prow = smem + AT_OFF_P + sb * AT_QTILE + r * 128;
-#pragma unroll
-      for (int c = 0; c < 8; ++c) {  // 8 keys -> one 16-byte chunk
-        uint32_t pk[4];
-#pragma unroll
-        for (int e = 0; e < 8; e += 2) {
-          const int i = c * 8 + e;
-          float x0, x1;
-          unpack2(fma2(pack2(__uint_as_float(s[i]), __uint_as_float(s[i + 1])), sl2, nm2), x0, x1);
-          float p0, p1;
-          if (POLY != 0 && (POLY == 1 ? (c & 3) == 3 : (POLY == 2 ? (c & 1) == 1 : (c & 3) != 0))) {
-            exp2_poly2(x0, x1, p0, p1);
-          } else {
-            p0 = ex2_approx(x0);
-            p1 = ex2_approx(x1);
-          }
-          if (TAIL) {
-            if (kbase + i >= ntok) p0 = 0.f;
-            if (kbase + i + 1 >= ntok) p1 = 0.f;
-          }
-          lsum = add2(lsum, pack2(p0, p1));
-          pk[e >> 1] = pack_bf16x2(p0, p1);
-        }
-        *reinterpret_cast<uint4*>(prow + ((c ^ sw) << 4)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-      }
-      float l0, l1;
-      unpack2(lsum, l0, l1);
-      l_run += l0 + l1;
-      fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core's async proxy
-      tc_fence_before();
-      mbar_arrive(&p_ready[sb]);
-    };
-
-    for (int j = 0; j < nkv; ++j) {
-      mbar_wait(&s_full[j & 1], (j >> 1) & 1);
-      tc_fence_after();
-      if (j * AT_BN + AT_BN > ntok) softmax_tile(j, std::true_type{});
-      else softmax_tile(j, std::false_type{});
+      msc[h] = m_run[h] * scale_log2e;
     }
-    // ---- O is complete after the last P V: normalise, store
-    {
-      const int pj = nkv - 1;
-      mbar_wait(&pv_done[pj & 1], (pj >> 1) & 1);
-      tc_fence_after();
-      const float inv = 1.0f / l_run;
-      const int row = q0 + r;
-      bf16* op = O + (static_cast<long long>(b) * ntok + row) * ldo + head * 64;
+    // P = exp2(s * scale - m * scale) as bf16 A fragments: k-chunk kk (keys 16 kk ..) = columns groups 2 kk, 2 kk + 1
+    uint32_t pa[4][4];
 #pragma unroll
-      for (int c2 = 0; c2 < 2; ++c2) {
-        uint32_t v[32];
-        tmem_ld32p(tO + lane_base + static_cast<uint32_t>(c2 * 32), v);
-        tmem_ld_wait();
-        if (row < ntok) {
+    for (int c = 0; c < 8; ++c) {
 #pragma unroll
-          for (int i = 0; i < 32; i += 8) {
-            uint32_t w[4];
-#pragma unroll
-            for (int e = 0; e < 8; e += 2)
-              w[e >> 1] = pack_bf16x2(__uint_as_float(v[i + e]) * inv, __uint_as_float(v[i + e + 1]) * inv);
-            *reinterpret_cast<uint4*>(op + c2 * 32 + i) = make_uint4(w[0], w[1], w[2], w[3]);
+      for (int h = 0; h < 2; ++h) {
+        const float x0 = fmaf(s[4 * c + 2 * h], scale_log2e, -msc[h]);
+        const float x1 = fmaf(s[4 * c + 2 * h + 1], scale_log2e, -msc[h]);
+        float p0, p1;
+        if (POLY != 0 && (POLY == 1 ? (c & 3) == 3 : (POLY == 2 ? (c & 1) == 1 : (c & 3) != 0))) {
+          exp2_poly2(x0, x1, p0, p1);
+          if (TAIL) {  // the polynomial clamps -inf to 2^-126
+            if (kbase + 8 * c + cq >= ntok) p0 = 0.f;
+            if (kbase + 8 * c + cq + 1 >= ntok) p1 = 0.f;
           }
+        } else {
+          p0 = ex2_approx(x0);
+          p1 = ex2_approx(x1);
         }
+        l_run[h] += p0 + p1;
+        pa[c >> 1][(c & 1) * 2 + h] = pack_bf16x2(p0, p1);
       }
+    }
+    const uint32_t vbase = smem_u32(smem + AT_OFF_V + st * AT_KTILE);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+      Wgmma<64>::rs(o, pa[kk], gmma_desc_mn_sw128(vbase + kk * 2048, AT_KTILE), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+  };
+
+  int st = 0;
+  uint32_t ph = 0;
+  for (int j = 0; j < nkv; ++j) {
+    mbar_wait(&kv_full[st], ph);
+    if (j * AT_BN + AT_BN > ntok) key_tile(j, st, std::true_type{});
+    else key_tile(j, st, std::false_type{});
+    if (wg_leader) mbar_arrive(&kv_empty[st]);
+    if (++st == AT_KVSTAGES) {
+      st = 0;
+      ph ^= 1u;
     }
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, AT_TMEM_COLS);
-  }
-}
-
-
-// ------------------------------------------------------------------------------------------------
-// NG query tiles per CTA (NG x 128 queries x one (sample, head)), ONE CTA per SM.
-//
-// What the one-tile kernel leaves on the table (ncu, profiles/ncu_r2_set_baseline_raw.csv): the MUFU pipe - the unit
-// that bounds a head-dim-64 softmax, 16 ex2 per clock per SM - is busy 58 % of the time, the tensor pipe 29 %, and the
-// FMA-pipe exp2 variants are SLOWER (profiles/microbench_r2_pair_rtma.md): the limit is not a pipe but the number of
-// softmax warps.  Two CTAs per SM give each SM sub-partition two of them, and a warp spends about as long outside its
-// exponentials (tcgen05.ld, row maximum, fences, barrier waits) as inside.  Registers are per sub-partition (16 K), so
-// more softmax warps means fewer registers each: this kernel runs NG = 3 groups of four softmax warps (12 + the TMA
-// and MMA warps = 14 warps, <= 128 registers) so that three warps per sub-partition interleave on the MUFU pipe.
-//   * group g owns query tile g: its score buffer S[g] (single: S_g(j+1) is issued as soon as the group holds S_g(j)
-//     in registers and completes far inside the 512 MUFU cycles of the tile), its two P operand tiles and its O
-//     accumulator in TMEM;
-//   * every K/V tile TMA brings in is shared by the NG tiles (a third of the K/V shared-memory traffic per query);
-//   * the tensor pipe alternates S_g(j+1), P_g(j) V(j) group by group in the order the groups finish.
-// TMEM: S[g] at columns g*64, O[g] at NG*64 + g*64 (384 of a 512-column allocation for NG = 3).
-// ------------------------------------------------------------------------------------------------
-constexpr int A2_KVSTAGES = 4;
-template <int NG>
-struct A2 {
-  static constexpr int BM = NG * AT_BM;
-  static constexpr int THREADS = 64 + 128 * NG;
-  static constexpr int OFF_Q = 0;                                          // NG x 16 KB
-  static constexpr int OFF_K = OFF_Q + NG * AT_QTILE;
-  static constexpr int OFF_V = OFF_K + A2_KVSTAGES * AT_KTILE;
-  static constexpr int OFF_P = OFF_V + A2_KVSTAGES * AT_KTILE;             // [g][b]: 2 NG x 16 KB
-  static constexpr int OFF_BAR = OFF_P + 2 * NG * AT_QTILE;
-  static constexpr int SMEM = OFF_BAR + 512;
-  static constexpr uint32_t TMEM_COLS = 512;
-};
-
-template <int NG>
-__global__ void __launch_bounds__(64 + 128 * NG, 1)
-attn_tcg_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                const __grid_constant__ CUtensorMap mapV, bf16* __restrict__ O, long long ldo, int ntok,
-                float scale_log2e) {
-  using C = A2<NG>;
-  extern __shared__ __align__(1024) uint8_t at_smem[];
-  uint8_t* smem = at_smem;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
-  uint64_t* q_full = bars + 0;
-  uint64_t* kv_full = bars + 1;                 // [4]
-  uint64_t* kv_empty = bars + 5;                // [4]
-  uint64_t* s_full = bars + 9;                  // [g]
-  uint64_t* s_empty = s_full + NG;              // [g]          128 arrivals
-  uint64_t* p_ready = s_empty + NG;             // [g*2 + b]    128 arrivals
-  uint64_t* pv_done = p_ready + 2 * NG;         // [g*2 + b]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(pv_done + 2 * NG);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * C::BM;
-  const int head = blockIdx.y;
-  const int b = blockIdx.z;
-  const int nkv = (ntok + AT_BN - 1) / AT_BN;
-
-  if (threadIdx.x == 0) {
-    if (smem_u32(smem) & 1023u) __trap();
-    tma_prefetch_desc(&mapQ);
-    tma_prefetch_desc(&mapK);
-    tma_prefetch_desc(&mapV);
-    mbar_init(q_full, 1);
-    for (int i = 0; i < A2_KVSTAGES; ++i) {
-      mbar_init(&kv_full[i], 1);
-      mbar_init(&kv_empty[i], 1);
+  // ---- normalise and store
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float l = l_run[h];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = 1.0f / l;
+    const int row = q0 + cw * 64 + wi * 16 + (lane >> 2) + 8 * h;
+    if (row < ntok) {
+      bf16* op = O + (static_cast<long long>(b) * ntok + row) * ldo + head * 64 + cq;
+#pragma unroll
+      for (int c = 0; c < 8; ++c)
+        *reinterpret_cast<uint32_t*>(op + 8 * c) = pack_bf16x2(o[4 * c + 2 * h] * inv, o[4 * c + 2 * h + 1] * inv);
     }
-    for (int i = 0; i < NG; ++i) {
-      mbar_init(&s_full[i], 1);
-      mbar_init(&s_empty[i], 128);
-    }
-    for (int i = 0; i < 2 * NG; ++i) {
-      mbar_init(&p_ready[i], 128);
-      mbar_init(&pv_done[i], 1);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, C::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      mbar_arrive_expect_tx(q_full, NG * AT_QTILE);
-#pragma unroll
-      for (int g = 0; g < NG; ++g)   // one 128-row box per tile (rows past ntok are zero-filled)
-        tma_load_3d(smem + C::OFF_Q + g * AT_QTILE, &mapQ, q_full, head * 64, q0 + g * AT_BM, b);
-      int st = 0;
-      uint32_t ph = 0;
-      for (int j = 0; j < nkv; ++j) {
-        mbar_wait(&kv_empty[st], ph ^ 1u);
-        mbar_arrive_expect_tx(&kv_full[st], 2 * AT_KTILE);
-        tma_load_3d(smem + C::OFF_K + st * AT_KTILE, &mapK, &kv_full[st], head * 64, j * AT_BN, b);
-        tma_load_3d(smem + C::OFF_V + st * AT_KTILE, &mapV, &kv_full[st], head * 64, j * AT_BN, b);
-        if (++st == A2_KVSTAGES) {
-          st = 0;
-          ph ^= 1u;
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = umma_idesc_bf16(128, 64, 0, 0);
-      constexpr uint32_t idesc_pv = umma_idesc_bf16(128, 64, 0, 1);
-      auto issue_s = [&](int g, int st) {
-        const uint64_t dq = umma_desc_k_sw128(smem_u32(smem + C::OFF_Q + g * AT_QTILE));
-        const uint64_t dk = umma_desc_k_sw128(smem_u32(smem + C::OFF_K + st * AT_KTILE));
-        const uint32_t d_s = tmem_base + static_cast<uint32_t>(g * 64);
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          tc_mma_f16(d_s, dq + static_cast<uint64_t>(2 * k), dk + static_cast<uint64_t>(2 * k), idesc_s, k != 0);
-        tc_commit(&s_full[g]);
-      };
-      mbar_wait(q_full, 0);
-      mbar_wait(&kv_full[0], 0);
-      tc_fence_after();
-#pragma unroll
-      for (int g = 0; g < NG; ++g) issue_s(g, 0);
-      int st = 0;
-      uint32_t ph = 0;
-      for (int j = 0; j < nkv; ++j) {
-        int st1 = st + 1;
-        uint32_t ph1 = ph;
-        if (st1 == A2_KVSTAGES) {
-          st1 = 0;
-          ph1 ^= 1u;
-        }
-        const bool more = j + 1 < nkv;
-        if (more) mbar_wait(&kv_full[st1], ph1);
-        const uint32_t vbase = smem_u32(smem + C::OFF_V + st * AT_KTILE);
-#pragma unroll
-        for (int g = 0; g < NG; ++g) {
-          // P_g(j) is written => the group also holds S_g(j) in registers: S[g] is free, and the group will come back
-          // for S_g(j+1) first, so that goes out before P_g(j) V(j)
-          mbar_wait(&p_ready[g * 2 + (j & 1)], (j >> 1) & 1);
-          if (more) {
-            mbar_wait(&s_empty[g], j & 1);
-            tc_fence_after();
-            issue_s(g, st1);
-          } else {
-            tc_fence_after();
-          }
-          const uint64_t dp0 = umma_desc_k_sw128(smem_u32(smem + C::OFF_P + (g * 2 + (j & 1)) * AT_QTILE));
-          const uint32_t t_o = tmem_base + static_cast<uint32_t>(NG * 64 + g * 64);
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {
-            const uint64_t dv = umma_desc_mn_sw128(vbase + kk * 2048, AT_KTILE);
-            tc_mma_f16(t_o, dp0 + static_cast<uint64_t>(2 * kk), dv, idesc_pv, (j | kk) != 0);
-          }
-          tc_commit(&pv_done[g * 2 + (j & 1)]);
-        }
-        tc_commit(&kv_empty[st]);
-        st = st1;
-        ph = ph1;
-      }
-    }
-  } else {
-    const int g = (warp - 2) >> 2;          // query tile of this softmax group
-    const int q = warp & 3;                 // TMEM lane quarter this warp may touch
-    const int r = q * 32 + lane;            // row inside the tile
-    const uint32_t lane_base = static_cast<uint32_t>(q * 32) << 16;
-    const uint32_t tS = tmem_base + static_cast<uint32_t>(g * 64);
-    const uint32_t tO = tmem_base + static_cast<uint32_t>(NG * 64 + g * 64);
-    uint64_t* pr = p_ready + g * 2;
-    uint64_t* pd = pv_done + g * 2;
-    const int sw = r & 7;
-    float m_ref = -INFINITY, l_run = 0.f;
-    const uint64_t sl2 = pack2(scale_log2e, scale_log2e);
-    // a tile of queries that lies entirely past ntok (last CTA of a sequence) still runs the protocol: its rows are
-    // zero-filled Q, and nothing is stored for them
-
-    auto softmax_tile = [&](int j, auto tail_tag) {
-      constexpr bool TAIL = decltype(tail_tag)::value;
-      const int kbase = j * AT_BN;
-      const int pb = j & 1;
-      uint32_t s[64];
-      tmem_ld32p(tS + lane_base, s);
-      tmem_ld32p(tS + lane_base + 32u, s + 32);
-      tmem_ld_wait();
-      tc_fence_before();
-      mbar_arrive(&s_empty[g]);  // the scores live in registers: S[g] may take tile j+1
-      // ---- row maximum: four independent chains
-      float mx4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-      for (int i = 0; i < 64; i += 2) {
-        float a0 = __uint_as_float(s[i]), a1 = __uint_as_float(s[i + 1]);
-        if (TAIL) {
-          if (kbase + i >= ntok) a0 = -INFINITY;
-          if (kbase + i + 1 >= ntok) a1 = -INFINITY;
-        }
-        mx4[(i >> 1) & 3] = fmaxf(fmaxf(a0, a1), mx4[(i >> 1) & 3]);
-      }
-      const float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-      if (j == 0) {
-        m_ref = mx;
-      } else {
-        const bool need = (mx - m_ref) * scale_log2e > AT_RESCALE_LOG2;
-        if (__any_sync(0xffffffffu, need)) {
-          float fac = 1.0f;
-          if (need) {
-            fac = ex2_approx((m_ref - mx) * scale_log2e);
-            m_ref = mx;
-          }
-          l_run *= fac;
-          mbar_wait(&pd[(j - 1) & 1], ((j - 1) >> 1) & 1);  // O holds tiles 0..j-1
-          tc_fence_after();
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            uint32_t o[16];
-            tmem_ld16p(tO + lane_base + static_cast<uint32_t>(c * 16), o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * fac);
-            tmem_st16p(tO + lane_base + static_cast<uint32_t>(c * 16), o);
-          }
-          tmem_st_wait();
-        }
-      }
-      if (j >= 2) mbar_wait(&pd[pb], ((j - 2) >> 1) & 1);   // P[g][pb] was last read by P_g(j-2) V(j-2)
-      const float msc = m_ref * scale_log2e;
-      const uint64_t nm2 = pack2(-msc, -msc);
-      uint64_t lsum = 0ull;
-      uint8_t* prow = smem + C::OFF_P + (g * 2 + pb) * AT_QTILE + r * 128;
-#pragma unroll
-      for (int c = 0; c < 8; ++c) {
-        uint32_t pk[4];
-#pragma unroll
-        for (int e = 0; e < 8; e += 2) {
-          const int i = c * 8 + e;
-          float x0, x1;
-          unpack2(fma2(pack2(__uint_as_float(s[i]), __uint_as_float(s[i + 1])), sl2, nm2), x0, x1);
-          float p0 = ex2_approx(x0), p1 = ex2_approx(x1);
-          if (TAIL) {
-            if (kbase + i >= ntok) p0 = 0.f;
-            if (kbase + i + 1 >= ntok) p1 = 0.f;
-          }
-          lsum = add2(lsum, pack2(p0, p1));
-          pk[e >> 1] = pack_bf16x2(p0, p1);
-        }
-        *reinterpret_cast<uint4*>(prow + ((c ^ sw) << 4)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-      }
-      float l0, l1;
-      unpack2(lsum, l0, l1);
-      l_run += l0 + l1;
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(&pr[pb]);
-    };
-
-    for (int j = 0; j < nkv; ++j) {
-      mbar_wait(&s_full[g], j & 1);
-      tc_fence_after();
-      if (j * AT_BN + AT_BN > ntok) softmax_tile(j, std::true_type{});
-      else softmax_tile(j, std::false_type{});
-    }
-    {
-      const int pj = nkv - 1;
-      mbar_wait(&pd[pj & 1], (pj >> 1) & 1);
-      tc_fence_after();
-      const float inv = 1.0f / l_run;
-      const int row = q0 + g * AT_BM + r;
-      bf16* op = O + (static_cast<long long>(b) * ntok + row) * ldo + head * 64;
-#pragma unroll
-      for (int c2 = 0; c2 < 2; ++c2) {
-        uint32_t v[32];
-        tmem_ld32p(tO + lane_base + static_cast<uint32_t>(c2 * 32), v);
-        tmem_ld_wait();
-        if (row < ntok) {
-#pragma unroll
-          for (int i = 0; i < 32; i += 8) {
-            uint32_t w[4];
-#pragma unroll
-            for (int e = 0; e < 8; e += 2)
-              w[e >> 1] = pack_bf16x2(__uint_as_float(v[i + e]) * inv, __uint_as_float(v[i + e + 1]) * inv);
-            *reinterpret_cast<uint4*>(op + c2 * 32 + i) = make_uint4(w[0], w[1], w[2], w[3]);
-          }
-        }
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, C::TMEM_COLS);
   }
 }
 
@@ -612,7 +226,7 @@ using namespace v3d;
 
 extern "C" {
 
-/* softmax(q k^T * scale) v per (sample, head), head dim 64, on tcgen05 tensor cores with TMA-staged operands.
+/* softmax(q k^T * scale) v per (sample, head), head dim 64, on wgmma tensor cores with TMA-staged operands.
  * q/k/v are column slices of one packed projection matrix (row stride ld_qkv elements), token rows sample-major.
  * Replaces F.scaled_dot_product_attention / xformers FMHA at sgm/modules/attention.py:337-341,432-444. */
 int v3d_attention_spatial(const void* q, const void* k, const void* v, void* o, int64_t ld_qkv, int64_t ld_o,
@@ -632,8 +246,8 @@ int v3d_attention_spatial(const void* q, const void* k, const void* v, void* o, 
   if ((rc = make_tmap_bf16(&mq, q, 3, dims, str, box_q))) return rc;
   if ((rc = make_tmap_bf16(&mk, k, 3, dims, str, box_kv))) return rc;
   if ((rc = make_tmap_bf16(&mv, v, 3, dims, str, box_kv))) return rc;
-  // V3D_ATTN_POLY = 1 | 2 | 3 (read once per process): opt-in FMA-pipe exp2 for 2 / 4 / 6 of a tile's 8 key chunks;
-  // not yet timed on hardware.  Default 0 = the validated kernel (its SASS is unchanged by the template).
+  // V3D_ATTN_POLY = 1 | 2 | 3 (read once per process): opt-in FMA-pipe exp2 for 2 / 4 / 6 of a tile's 8 key chunks.
+  // Default 0 = MUFU ex2 only.
   static int poly = -1;
   if (poly < 0) {
     const char* v = getenv("V3D_ATTN_POLY");
@@ -650,36 +264,6 @@ int v3d_attention_spatial(const void* q, const void* k, const void* v, void* o, 
       return V3D_ERR_CUDA;
     }
     cfg[poly] = true;
-  }
-  // V3D_ATTN_TILES = 1 (default) | 2 | 3: query tiles per CTA.  1 = the one-tile kernel, two CTAs per SM; 2 / 3 =
-  // attn_tcg_kernel<NG> (one CTA per SM, NG softmax groups sharing the K/V tiles) for sequences of at least NG * 128
-  // tokens - validated, but SLOWER on hardware (641 vs 531 / 571 TFLOP/s at 4096 tokens, profiles/microbench_r2_attn_norm.md):
-  // the softmax warps are bound by fixed-latency dependency stalls, not by the number of warps per sub-partition
-  static int tiles = -1;
-  if (tiles < 0) {
-    const char* v = getenv("V3D_ATTN_TILES");
-    tiles = v ? atoi(v) : 1;
-    if (tiles < 1 || tiles > 3) tiles = 1;
-  }
-  if (tiles >= 2 && poly == 0 && ntok >= 2 * AT_BM) {
-    const int ng = (tiles == 3 && ntok >= 3 * AT_BM) ? 3 : 2;
-    using Kern2 = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, bf16*, long long, int, float);
-    const Kern2 k2 = ng == 3 ? static_cast<Kern2>(attn_tcg_kernel<3>) : static_cast<Kern2>(attn_tcg_kernel<2>);
-    const int smem2 = ng == 3 ? A2<3>::SMEM : A2<2>::SMEM;
-    static bool cfg2[4] = {false, false, false, false};
-    if (!cfg2[ng]) {
-      cudaError_t e = cudaFuncSetAttribute(k2, cudaFuncAttributeMaxDynamicSharedMemorySize, smem2);
-      if (e != cudaSuccess) {
-        set_error("attn_tcg smem attr: %s", cudaGetErrorString(e));
-        return V3D_ERR_CUDA;
-      }
-      cfg2[ng] = true;
-    }
-    dim3 grid2((ntok + ng * AT_BM - 1) / (ng * AT_BM), nheads, nbatch);
-    k2<<<grid2, 64 + 128 * ng, smem2, static_cast<cudaStream_t>(stream)>>>(
-        mq, mk, mv, static_cast<bf16*>(o), ld_o, ntok, scale * 1.44269504088896340736f);
-    V3D_CHECK_LAUNCH("attn_tcg_kernel");
-    return V3D_OK;
   }
   dim3 grid((ntok + AT_BM - 1) / AT_BM, nheads, nbatch);
   kerns[poly]<<<grid, AT_THREADS, AT_SMEM, static_cast<cudaStream_t>(stream)>>>(

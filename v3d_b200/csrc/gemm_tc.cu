@@ -1,11 +1,12 @@
-// tcgen05 GEMM / temporal-conv / implicit-GEMM 3x3 conv for sm_100a.
+// wgmma GEMM / temporal-conv / implicit-GEMM 3x3 conv for sm_90a.
 //
-// One persistent, warp-specialised kernel:
-//   warp 0      : TMA producer  (A tile 128x64 bf16 + B tile BNx64 bf16 per pipeline stage, 128B swizzle)
-//   warp 1      : TMEM allocator + single-thread tcgen05.mma issuer (128 x BN x 16 per instruction)
-//   warps 2..9  : epilogue (tcgen05.ld 32x32b -> bias / per-frame bias / SiLU / GEGLU / residual blend ->
-//                 bf16 or fp32 stores). Two TMEM accumulator stages so the epilogue of tile i overlaps
-//                 the main loop of tile i+1.
+// One persistent, warp-specialised kernel, 128 x BN output tiles:
+//   warpgroup 0    : TMA producer (one thread; A tile 128x64 bf16 + B tile BNx64 bf16 per pipeline stage, 128B swizzle)
+//   warpgroups 1-2 : consumers.  Each owns 64 rows of the tile: wgmma.mma_async m64nBNk16 from shared memory into
+//                    fp32 register accumulators, then the epilogue straight from those registers (bias / per-frame
+//                    bias / SiLU / GEGLU / residual blend -> bf16 sub-tiles staged in shared memory and written by TMA,
+//                    or fp32 stores).  While the consumers run the epilogue the producer already fills the ring with
+//                    the next tile's operands.
 // Operand gather modes (see include/v3d_b200.h): linear rows, 3-tap temporal shift, 3x3 spatial taps.
 // The im2row never exists in memory: each (tap, 64-channel) K-block is one TMA box whose out-of-bounds
 // part is zero-filled by the hardware, which is exactly the conv zero padding.
@@ -14,12 +15,14 @@
 #include "common.cuh"
 #include "host_util.cuh"
 #include "v3d_b200.h"
+#include "wgmma.cuh"
 
 namespace v3d {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int kThreads = 320;  // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue
+constexpr int kThreads = 384;  // warpgroup 0 TMA, warpgroups 1 and 2 MMA + epilogue
+constexpr int kConsumerThreads = 256;
 constexpr int kSmemBudget = 227 * 1024;
 
 struct GemmEpi {
@@ -33,11 +36,6 @@ struct GemmEpi {
   int N, kpt, ntaps, tap_shift;  // kpt = K-blocks per tap
   int rows_per_frame, act, out_fp32;
   int b_batched;
-  int fb_uniform;  // every 32-row warp slice of a tile lies in one frame: per-frame bias folds into the bias registers
-  long long* trace;  // diagnostics only: CTA 0 writes role timelines (clock64) here when non-null
-  // diagnostics only (V3D_GEMM_DEBUG): 1 = skip the store path, 2 = skip TMA store issue, 4 = skip TMEM loads,
-  // 8 = skip the drain wait, 16 = skip the proxy fence, 32 = skip the smem writes.  Results are wrong with any bit set.
-  int dbg;
   int transposed, valid_cols, accumulate;  // small-M mode: D is fp32 [cols][ldd], D[col][row]; bias per row
   // conv3x3 geometry
   int cn, ch, cw, bw, bh, bn, tiles_w, tiles_h, bw_shift, bh_shift, tw_shift, th_shift;  // t*_shift < 0: not pow2
@@ -56,57 +54,40 @@ struct alignas(64) KvMaps {
   int col0;
 };
 
-// Diagnostics (role timelines through v3d_debug_set_trace, V3D_GEMM_DEBUG stage-skipping switches) are compiled in
-// only with -DV3D_GEMM_DIAG: the hooks cost registers and ~6% of the epilogue's issue slots.
-#ifdef V3D_GEMM_DIAG
-#define V3D_DIAG(x) (x)
-#define V3D_DBG(bit) (p.dbg & (bit))
-#else
-#define V3D_DIAG(x) (false)
-#define V3D_DBG(bit) (0)
-#endif
-
-// NCTA = 1: one CTA per 128-row tile.  NCTA = 2: a CTA pair (cluster of 2, cta_group::2) computes a 256 x BN tile;
-// each CTA stages its own 128 rows of A and HALF of the B tile, the leader's tensor core reads both halves.
-template <int BN, int NCTA = 1, bool RT = false>
-struct Cfg {
-  static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = (BN / NCTA) * BK * 2;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  // 4 KB per epilogue warp: 32 rows x 128 B, swizzled; RT adds a ring of RDEPTH residual sub-tiles (8 KB each) per group
-  static constexpr int OUT_STAGING_BYTES = 8 * 4096;
-  static constexpr int RDEPTH = 3;
-  static constexpr int STAGING_BYTES = OUT_STAGING_BYTES + (RT ? 2 * RDEPTH * 8192 : 0);
-  static constexpr int NSTAGE_RAW = (kSmemBudget - 2048 - STAGING_BYTES) / STAGE_BYTES;
-  static constexpr int NSTAGE = NSTAGE_RAW > 8 ? 8 : NSTAGE_RAW;
-  // accumulator ring in TMEM: as many stages as fit in the 512 columns (max 4). Deeper rings let the MMA issuer run
-  // further ahead of the epilogue, which hides the tile-to-tile signalling round trip on short-K problems.
-  static constexpr int ACC_STRIDE = BN <= 32 ? 32 : (BN <= 64 ? 64 : (BN <= 128 ? 128 : (BN <= 160 ? 160 : 256)));
-  static constexpr int ACC_STAGES = (512 / ACC_STRIDE) > 4 ? 4 : (512 / ACC_STRIDE);
-  static constexpr int TMEM_COLS = 512;
-  static constexpr int SMEM_BYTES = NSTAGE * STAGE_BYTES + STAGING_BYTES + 1024 /*align slack*/ + (RT ? 512 : 256) /*barriers*/;
-};
-
 // epilogue variants (compile-time): what is stored and how
 constexpr int EPI_BF16 = 0;   // bf16 sub-tiles staged in shared memory, written by TMA; at most one residual (R1)
 constexpr int EPI_BF16R2 = 4; // as EPI_BF16 with both residuals (blend epilogue); the only variant that carries R2
-constexpr int EPI_BF16RT = 5; // as EPI_BF16 with R1 always present and staged by TMA: the residual sub-tile (128 rows x 32
-                              // columns) lands in shared memory two sub-tiles ahead of its use instead of arriving
-                              // through per-lane global loads one load group ahead (opt-in: V3D_GEMM_RTMA=1)
 constexpr int EPI_GEGLU = 1;  // value * gelu(gate) then as EPI_BF16 (linear mode only)
 constexpr int EPI_F32 = 2;    // fp32 direct stores (optional SiLU)
 constexpr int EPI_TRANS = 3;  // fp32 transposed store with per-row bias (small-M mode, linear only)
 
-// Persistent tile walk without per-tile divisions: tile = first + i * step, n fastest.  With CTA pairs the walk is
-// over pair tiles (m_tile = pair index; the CTA's own 128-row tile is 2 * m_tile + rank).
+template <int BN, int EPI>
+struct Cfg {
+  static constexpr bool STAGED = EPI == EPI_BF16 || EPI == EPI_BF16R2 || EPI == EPI_GEGLU;
+  static constexpr int OUT_COLS = EPI == EPI_GEGLU ? BN / 2 : BN;
+  // bf16 output leaves as 128-row x SUBW-column TMA stores (64B-swizzled rows when SUBW = 32)
+  static constexpr int SUBW = OUT_COLS % 32 == 0 ? 32 : 16;
+  static constexpr int NSUB = OUT_COLS / SUBW;
+  static constexpr int SUB_BYTES = BM * SUBW * 2;
+  static constexpr int A_BYTES = BM * BK * 2;
+  static constexpr int B_BYTES = BN * BK * 2;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int STAGING_BYTES = STAGED ? NSUB * SUB_BYTES : 0;
+  static constexpr int NSTAGE_RAW = (kSmemBudget - 2048 - STAGING_BYTES) / STAGE_BYTES;
+  static constexpr int NSTAGE = NSTAGE_RAW > 8 ? 8 : NSTAGE_RAW;
+  static constexpr int SMEM_BYTES = NSTAGE * STAGE_BYTES + STAGING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(NSTAGE >= 2, "pipeline too shallow");
+};
+
+// Persistent tile walk without per-tile divisions: tile = first + i * step, n fastest.
 struct TileWalk {
   int n_tile, m_tile, step_n, step_m, num_n;
-  __device__ __forceinline__ TileWalk(const GemmEpi& p, int ncta) {
+  __device__ __forceinline__ explicit TileWalk(const GemmEpi& p) {
     num_n = p.num_n_tiles;
-    n_tile = (static_cast<int>(blockIdx.x) / ncta) % num_n;
-    m_tile = (static_cast<int>(blockIdx.x) / ncta) / num_n;
-    step_n = (static_cast<int>(gridDim.x) / ncta) % num_n;
-    step_m = (static_cast<int>(gridDim.x) / ncta) / num_n;
+    n_tile = static_cast<int>(blockIdx.x) % num_n;
+    m_tile = static_cast<int>(blockIdx.x) / num_n;
+    step_n = static_cast<int>(gridDim.x) % num_n;
+    step_m = static_cast<int>(gridDim.x) / num_n;
   }
   __device__ __forceinline__ void next() {
     n_tile += step_n;
@@ -147,111 +128,59 @@ __device__ __forceinline__ void tile_origin(const GemmEpi& p, int m_tile, int& t
   }
 }
 
-template <int BN, bool CONV, int EPI, int NCTA = 1>
+template <int BN, bool CONV, int EPI>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
-               const __grid_constant__ CUtensorMap mapD, const GemmEpi p, const __grid_constant__ CUtensorMap mapR,
-               const __grid_constant__ KvMaps kv) {
-  constexpr bool RTMA = EPI == EPI_BF16RT;
-  static_assert(!RTMA || NCTA == 1, "the TMA-staged residual variant is single-CTA");
-  using C = Cfg<BN, NCTA, RTMA>;
-  static_assert(NCTA == 1 || NCTA == 2, "one CTA or a CTA pair");
+               const __grid_constant__ CUtensorMap mapD, const GemmEpi p, const __grid_constant__ KvMaps kv) {
+  using C = Cfg<BN, EPI>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* staging = smem + C::NSTAGE * C::STAGE_BYTES;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + C::STAGING_BYTES);
   uint64_t* empty_bar = full_bar + C::NSTAGE;
-  uint64_t* tfull_bar = empty_bar + C::NSTAGE;
-  uint64_t* tempty_bar = tfull_bar + 4;
-  uint64_t* rfull_bar = tempty_bar + 4;  // RTMA only: [group][ring slot], one TMA transaction each
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 4 + (RTMA ? 2 * C::RDEPTH : 0));
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&mapA);
     tma_prefetch_desc(&mapB);
-    if (EPI == EPI_BF16 || EPI == EPI_BF16R2 || EPI == EPI_GEGLU || RTMA) tma_prefetch_desc(&mapD);
-    if (RTMA) {
-      tma_prefetch_desc(&mapR);
-      for (int i = 0; i < 2 * C::RDEPTH; ++i) mbar_init(&rfull_bar[i], 1);
-    }
+    if (C::STAGED) tma_prefetch_desc(&mapD);
     for (int i = 0; i < C::NSTAGE; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < C::ACC_STAGES; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 8 * NCTA);  // pair: the leader's barrier collects both CTAs' epilogue warps
+      mbar_init(&empty_bar[i], 2);  // one arrival per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    if (NCTA == 2) {
-      tmem_alloc_2cta(tmem_slot, C::TMEM_COLS);
-      tmem_relinquish_2cta();
-    } else {
-      tmem_alloc(tmem_slot, C::TMEM_COLS);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  if (NCTA == 2) cluster_sync_all();  // both CTAs' barriers exist before any remote arrive / TMA credit
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // rank inside the pair; the persistent walk is over pair tiles: first = blockIdx.x / NCTA, step = gridDim.x / NCTA
-  const int cta_rank = NCTA == 2 ? static_cast<int>(cluster_ctarank()) : 0;
-  const int total_tiles = ((p.num_m_tiles + NCTA - 1) / NCTA) * p.num_n_tiles;
+  const int total_tiles = p.num_m_tiles * p.num_n_tiles;
   const int num_kb = p.ntaps * p.kpt;
 
-  if (warp == 0) {
+  if (threadIdx.x < 128) {
     // ------------------------------ TMA producer ------------------------------
-    if (lane == 0) {
+    regs_dec<40>();
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      int tr_n = 0;
-      TileWalk tw(p, NCTA);
-      for (int tile = blockIdx.x / NCTA; tile < total_tiles; tile += gridDim.x / NCTA, tw.next()) {
-        const int n_tile = tw.n_tile;
-        const int m_tile = tw.m_tile * NCTA + cta_rank;
+      TileWalk tw(p);
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, tw.next()) {
         int c1, c2, c3;
-        if (CONV) {
-          tile_origin<true>(p, m_tile, c1, c2, c3);
-        } else {
-          tile_origin<false>(p, m_tile, c2, c1, c3);
-        }
+        if (CONV) tile_origin<true>(p, tw.m_tile, c1, c2, c3);
+        else tile_origin<false>(p, tw.m_tile, c2, c1, c3);
         const int bz = p.b_batched ? c2 : 0;
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1u);
-          if (V3D_DIAG(p.trace && blockIdx.x == 0 && tr_n < 1024)) p.trace[tr_n++] = clock64();
           uint8_t* sa = smem + stage * C::STAGE_BYTES;
           uint8_t* sb = sa + C::A_BYTES;
-          // pair: only the leader arms its barrier, with the bytes of both CTAs; the peer's loads credit it remotely
-          if (NCTA == 1 || cta_rank == 0) mbar_arrive_expect_tx(&full_bar[stage], NCTA * C::STAGE_BYTES);
+          mbar_arrive_expect_tx(&full_bar[stage], C::STAGE_BYTES);
           const int tap = kb / p.kpt;
           const int kc = (kb - tap * p.kpt) * BK;
-          if (NCTA == 2) {
-            if (CONV) {
-              const int ky = tap / 3, kx = tap - ky * 3;
-              tma_load_4d_2cta(sa, &mapA, &full_bar[stage], kc, c1 + kx - 1, c2 + ky - 1, c3);
-            } else {
-              tma_load_3d_2cta(sa, &mapA, &full_bar[stage], kc, c1 + tap * p.tap_shift + p.tap0, c2);
-            }
-            // this CTA's half of the B tile: rows [rank * BN/2, (rank + 1) * BN/2) of the N tile
-            tma_load_3d_2cta(sb, &mapB, &full_bar[stage], kb * BK, n_tile * BN + cta_rank * (BN / 2), bz);
+          if (CONV) {
+            const int ky = tap / 3, kx = tap - ky * 3;
+            tma_load_4d(sa, &mapA, &full_bar[stage], kc, c1 + kx - 1, c2 + ky - 1, c3);
           } else {
-            if (CONV) {
-              const int ky = tap / 3, kx = tap - ky * 3;
-              tma_load_4d(sa, &mapA, &full_bar[stage], kc, c1 + kx - 1, c2 + ky - 1, c3);
-            } else {
-              tma_load_3d(sa, &mapA, &full_bar[stage], kc, c1 + tap * p.tap_shift + p.tap0, c2);
-            }
-            tma_load_3d(sb, &mapB, &full_bar[stage], kb * BK, n_tile * BN, bz);
+            tma_load_3d(sa, &mapA, &full_bar[stage], kc, c1 + tap * p.tap_shift + p.tap0, c2);
           }
+          tma_load_3d(sb, &mapB, &full_bar[stage], kb * BK, tw.n_tile * BN, bz);
           if (++stage == C::NSTAGE) {
             stage = 0;
             phase ^= 1u;
@@ -259,467 +188,203 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer ------------------------------
-    if (lane == 0 && (NCTA == 1 || cta_rank == 0)) {  // pair: the leader issues for both SMs
-      constexpr uint32_t idesc = umma_idesc_bf16(BM * NCTA, BN, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      int tr_m = 0;
-      for (int tile = blockIdx.x / NCTA; tile < total_tiles; tile += gridDim.x / NCTA) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1u);
-        tc_fence_after();
-        if (V3D_DIAG(p.trace && blockIdx.x == 0 && tr_m < 1020)) p.trace[1024 + tr_m++] = -clock64();  // negative: tile start
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(acc * C::ACC_STRIDE);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          if (V3D_DIAG(p.trace && blockIdx.x == 0 && tr_m < 1020)) p.trace[1024 + tr_m++] = clock64();
-          const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES);
-          const uint64_t adesc = umma_desc_k_sw128(sa);
-          const uint64_t bdesc = umma_desc_k_sw128(sa + C::A_BYTES);
+    return;
+  }
+
+  // ------------------------------ consumers: MMA + epilogue ------------------------------
+  regs_inc<232>();
+  constexpr bool GEGLU = EPI == EPI_GEGLU;
+  constexpr bool DUAL = EPI == EPI_BF16R2 || EPI == EPI_F32;  // variants that may take a second residual
+  constexpr int OUT_COLS = C::OUT_COLS;
+  constexpr int SUBW = C::SUBW;
+  const int ct = threadIdx.x - 128;       // 0..255
+  const int cw = ct >> 7;                 // consumer warpgroup: tile rows [64 cw, 64 cw + 64)
+  const int wi = (ct >> 5) & 3;           // warp inside the warpgroup: 16 of those rows
+  const int lane = ct & 31;
+  const bool wg_leader = (ct & 127) == 0;
+  const bool store_leader = ct == 0;
+  const int cq = (lane & 3) * 2;          // first of the thread's two columns inside each 8-column group
+  const int tr_base = cw * 64 + wi * 16 + (lane >> 2);  // tile rows tr_base and tr_base + 8
+  const bool has_bias = p.bias != nullptr;
+  // the GEGLU variant carries no residual / per-frame bias code (rejected on the host): registers
+  const bool has_fb = !GEGLU && p.fbias != nullptr;
+  const bool has_r1 = !GEGLU && p.R1 != nullptr;
+  const bool has_r2 = DUAL && p.R2 != nullptr;
+  const bool do_silu = p.act == V3D_ACT_SILU;
+  const float s0 = p.s0, s1 = p.s1, s2 = p.s2;
+  const uint32_t stg = smem_u32(staging);
+
+  // tile row -> (valid, global row). bw/bh are powers of two (checked on the host).
+  auto map_row = [&](int tr, int o0, int o1, int o2, long long& grow) -> bool {
+    if (CONV) {
+      const int w = tr & (p.bw - 1);
+      const int h = (tr >> p.bw_shift) & (p.bh - 1);
+      const int img = o2 + (tr >> (p.bw_shift + p.bh_shift));
+      grow = (static_cast<long long>(img) * p.ch + (o1 + h)) * p.cw + (o0 + w);
+      return img < p.cn;
+    } else {
+      const int m = o1 + tr;
+      grow = static_cast<long long>(o0) * p.rows_per_batch + m;
+      return m < p.rows_per_batch;
+    }
+  };
+
+  float acc[BN / 2];
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            // +32 bytes per 16-element K step inside the 128B swizzle atom (encoded >>4)
-            if (NCTA == 2)
-              tc_mma_f16_2cta(d_tmem, adesc + static_cast<uint64_t>(k * 2), bdesc + static_cast<uint64_t>(k * 2),
-                              idesc, (kb | k) != 0 ? 1u : 0u);
-            else
-              tc_mma_f16(d_tmem, adesc + static_cast<uint64_t>(k * 2), bdesc + static_cast<uint64_t>(k * 2),
-                         idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          if (NCTA == 2) tc_commit_2cta(&empty_bar[stage], 3);  // frees the stage in both CTAs
-          else tc_commit(&empty_bar[stage]);
-          if (++stage == C::NSTAGE) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-        if (NCTA == 2) tc_commit_2cta(&tfull_bar[acc], 3);  // each CTA's epilogue reads its own 128 rows
-        else tc_commit(&tfull_bar[acc]);
-        if (++acc == C::ACC_STAGES) {
-          acc = 0;
-          acc_phase ^= 1u;
-        }
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  int stage = 0;
+  uint32_t phase = 0;
+  TileWalk tw(p);
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const int n_tile = tw.n_tile;
+    int t0, t1, t2;
+    tile_origin<CONV>(p, tw.m_tile, t0, t1, t2);
+    tw.next();
+
+    // ---- main loop: one wgmma group per K-block; the stage of block kb-1 is released once block kb is issued
+    int prev = -1;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES);
+      const uint64_t adesc = gmma_desc_k_sw128(sa + static_cast<uint32_t>(cw * 64 * 128));
+      const uint64_t bdesc = gmma_desc_k_sw128(sa + C::A_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k)
+        Wgmma<BN>::ss(acc, adesc + static_cast<uint64_t>(2 * k), bdesc + static_cast<uint64_t>(2 * k),
+                      (kb | k) != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0 && wg_leader) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == C::NSTAGE) {
+        stage = 0;
+        phase ^= 1u;
       }
     }
-  } else {
-    // ------------------------------ epilogue (warps 2..9) ------------------------------
-    // Two warps per TMEM lane quarter; each takes half of the tile's 16-column chunks.  The variant (EPI) is a
-    // template parameter and the chunk loop is fully unrolled, so the per-chunk code is straight-line: TMEM load,
-    // bias/residual loads issued underneath it, math, then either the swizzled smem slab (32 rows x 128 B per
-    // warp, flushed as row-contiguous 16-byte stores: 4 full 128-byte lines per warp instruction) or direct fp32.
-    constexpr bool GEGLU = EPI == EPI_GEGLU;
-    constexpr bool STAGED = EPI == EPI_BF16 || EPI == EPI_BF16R2 || EPI == EPI_GEGLU || RTMA;
-    constexpr bool DUAL = EPI == EPI_BF16R2 || EPI == EPI_F32;  // variants that may take a second residual
-    constexpr int OUT_COLS = GEGLU ? BN / 2 : BN;
-    constexpr int NCH = OUT_COLS / 16;
-    // bf16 output leaves as whole-tile-height TMA stores: a sub-tile is 128 rows x SUBW columns, staged by the four
-    // warps of a group (one per TMEM lane quarter) in one of the group's two buffers and written by one
-    // cp.async.bulk.tensor per sub-tile.  Group 0 (warps 2..5) takes the first half of the sub-tiles, group 1 the rest.
-    constexpr int SUBW = (STAGED && OUT_COLS % 32 == 0) ? 32 : 16;
-    constexpr int CPS = SUBW / 16;  // 16-column chunks per sub-tile
-    constexpr int NSUB = OUT_COLS / SUBW;
-    constexpr int CH_HALF = ((NSUB + 1) / 2) * CPS;
-    constexpr int SUB_BYTES = BM * SUBW * 2;
-    static_assert(2 * 2 * SUB_BYTES <= C::OUT_STAGING_BYTES, "staging too small");
-    static_assert(!RTMA || SUBW == 32, "the TMA-staged residual needs 32-column sub-tiles");
-    const int q = warp & 3;             // TMEM lane quarter this warp may access
-    const int half = (warp - 2) >> 2;   // 0: warps 2..5, 1: warps 6..9
-    const int r = q * 32 + lane;
-    const uint32_t stg = smem_u32(staging) + static_cast<uint32_t>(half * 2 * SUB_BYTES);  // this group's buffers
-    // RTMA: this group's ring of residual buffers (same 128 x 64 B, 64B-swizzled layout as the output buffers) and
-    // their barriers; sub-tile number n (the group's running count `nstore`) lives in slot n % RD, phase (n / RD) & 1
-    constexpr uint32_t RD = C::RDEPTH;
-    uint8_t* const rbuf = staging + C::OUT_STAGING_BYTES + half * static_cast<int>(RD) * SUB_BYTES;
-    uint64_t* const rfull = rfull_bar + half * RD;
-    const bool store_leader = q == 0 && lane == 0;
-    const uint32_t row_off = static_cast<uint32_t>(r * SUBW * 2);
-    const uint32_t swz = SUBW == 32 ? static_cast<uint32_t>((r >> 1) & 3) : 0u;  // 64B-swizzle XOR of the 16-byte chunk
-    const bool has_bias = p.bias != nullptr;
-    // the GEGLU variant carries no residual / per-frame bias code (rejected on the host): registers
-    const bool has_fb = !GEGLU && p.fbias != nullptr;
-    const bool has_r1 = !GEGLU && p.R1 != nullptr;
-    const bool has_r2 = DUAL && p.R2 != nullptr;
-    const bool do_silu = p.act == V3D_ACT_SILU;
-    const float s0 = p.s0, s1 = p.s1, s2 = p.s2;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    uint32_t nstore = 0;  // sub-tiles this group has stored (buffer ring position)
-    int tr_e = 0;
-    const bool tracing = V3D_DIAG(p.trace && blockIdx.x == 0 && warp == 4 && lane == 0);  // group 0's store leader
-#define V3D_ETRACE() do { if (V3D_DIAG(tracing && tr_e < 1020)) p.trace[2048 + tr_e++] = clock64(); } while (0)
-    // TMEM is read in load groups, double-buffered: while one group is processed the next is in flight.  A group is
-    // a whole sub-tile (32 columns, one x32 load) for bf16 output, value+gate (2 x16) for GEGLU, one x16 otherwise.
-    constexpr int LG = GEGLU ? 1 : CPS;          // 16-column output chunks per load group
-    constexpr int LREGS = GEGLU ? 32 : 16 * LG;  // registers per buffer
-    constexpr int NG_HALF = CH_HALF / LG;
-    constexpr int NBR = (CH_HALF * 16 + 31) / 32;  // bias registers per lane
-    // tile row -> (valid, global row). bw/bh are powers of two (checked on the host).
-    auto map_row_of = [&](int tr, int o0, int o1, int o2, long long& grow) -> bool {
-      if (CONV) {
-        const int w = tr & (p.bw - 1);
-        const int h = (tr >> p.bw_shift) & (p.bh - 1);
-        const int img = o2 + (tr >> (p.bw_shift + p.bh_shift));
-        grow = (static_cast<long long>(img) * p.ch + (o1 + h)) * p.cw + (o0 + w);
-        return img < p.cn;
-      } else {
-        const int m = o1 + tr;
-        grow = static_cast<long long>(o0) * p.rows_per_batch + m;
-        // pair: with an odd number of 128-row tiles the peer's last tile lies past the last batch item (its TMA
-        // loads are zero-filled and its stores clipped; its residual / per-frame-bias rows must not be touched)
-        return m < p.rows_per_batch && (NCTA == 1 || o0 < p.batch);
-      }
-    };
-    TileWalk tw(p, NCTA);
-    int iter = 0;
-    for (int tile = blockIdx.x / NCTA; tile < total_tiles; tile += gridDim.x / NCTA, ++iter) {
-      V3D_ETRACE();  // [0] tile prologue start
-      const int n_tile = tw.n_tile;
-      int t0, t1, t2;
-      tile_origin<CONV>(p, tw.m_tile * NCTA + cta_rank, t0, t1, t2);
-      tw.next();  // tw now names the next tile (used by the residual prefetch below)
-      // with an odd number of sub-tiles the two groups swap the larger share every tile, so neither paces the other
-      const int hsel = (NSUB & 1) ? (half ^ (iter & 1)) : half;
-      const int c_begin = hsel ? CH_HALF : 0;
-      const int my_n = hsel ? NCH - CH_HALF : CH_HALF;
-      const int c_begin_next = (NSUB & 1) ? (hsel ? 0 : CH_HALF) : c_begin;
+    wgmma_wait<0>();
+    if (prev >= 0 && wg_leader) mbar_arrive(&empty_bar[prev]);
 
-      // accumulator first: the first TMEM load is in flight while the row bookkeeping below is computed
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      V3D_ETRACE();  // [1] accumulator ready
-      const uint32_t t_acc =
-          tmem_base + static_cast<uint32_t>(acc * C::ACC_STRIDE) + (static_cast<uint32_t>(q * 32) << 16);
-      uint32_t vb[2][LREGS];
-      auto issue_group = [&](int g, uint32_t* dst) {
-        if (V3D_DBG(4)) return;
-        const uint32_t c = static_cast<uint32_t>((c_begin + g * LG) * 16);
-        if (GEGLU) {
-          tmem_ld16p(t_acc + c, dst);
-          tmem_ld16p(t_acc + static_cast<uint32_t>(BN / 2) + c, dst + 16);
-        } else if (LG == 2) {
-          tmem_ld32p(t_acc + c, dst);
-        } else {
-          tmem_ld16p(t_acc + c, dst);
-        }
-      };
-      if (my_n > 0) issue_group(0, vb[0]);
-      // bias for this warp's columns, one coalesced load per tile, spread over the lanes (column i*32+lane of the
-      // warp's slice) and handed out by shuffles in the chunk loop: no memory latency inside the loop.  A per-frame
-      // bias that is uniform over the warp's rows is folded in here.
-      float breg[NBR], greg[GEGLU ? NBR : 1];
-      {
-        const float* fbw = nullptr;
-        if (has_fb && p.fb_uniform) {
-          long long rw;
-          if (map_row_of(q * 32, t0, t1, t2, rw))
-            fbw = p.fbias + static_cast<long long>(static_cast<int>(rw) / p.rows_per_frame) * p.ldfb + n_tile * BN;
-        }
+    // ---- epilogue from registers.  acc[4 j + 2 h + e] = tile row tr_base + 8 h, column 8 j + cq + e.
+    if (C::STAGED) {
+      // the previous tile's TMA stores must have finished reading the staging buffer
+      if (store_leader) bulk_wait_read<0>();
+      asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory");
+    }
+    const int obase = n_tile * OUT_COLS;  // first output column of this tile
+    const int nbase = n_tile * BN;        // first column in the (packed) N space
 #pragma unroll
-        for (int i = 0; i < NBR; ++i) {
-          const int col = c_begin * 16 + i * 32 + lane;
-          const bool ok = i * 32 + lane < my_n * 16;
-          float bvv = 0.f;
-          if (EPI != EPI_TRANS && has_bias && ok) bvv = __ldg(p.bias + n_tile * BN + col);
-          if (fbw && ok) bvv += __ldg(fbw + col);
-          breg[i] = bvv;
-          if (GEGLU) greg[i] = (has_bias && ok) ? __ldg(p.bias + n_tile * BN + BN / 2 + col) : 0.f;
-        }
-      }
-
-      // tile row -> (valid, global row). bw/bh are powers of two (checked on the host).
-      auto map_row = [&](int o0, int o1, int o2, long long& grow) -> bool {
-        return map_row_of(r, o0, o1, o2, grow);
-      };
-      const int obase = n_tile * OUT_COLS;  // first output column of this tile
-      const int nbase = n_tile * BN;        // first column in the (packed) N space
+    for (int h = 0; h < 2; ++h) {
+      const int tr = tr_base + 8 * h;
       long long row = 0;
-      bool valid = true;
+      const bool valid = map_row(tr, t0, t1, t2, row);
       const float* fb = nullptr;
       const bf16* r1p = nullptr;
       const bf16* r2p = nullptr;
       float row_bias = 0.f;
-      if (!STAGED || (has_fb && !p.fb_uniform) || has_r1 || has_r2) {  // plain bf16 tiles never need per-row addresses
-        valid = map_row(t0, t1, t2, row);
-        if (has_fb && !p.fb_uniform && valid) fb = p.fbias + static_cast<long long>(static_cast<int>(row) / p.rows_per_frame) * p.ldfb + nbase;
-        if (has_r1 && valid) r1p = p.R1 + row * p.ldr1 + obase;
-        if (has_r2 && valid) r2p = p.R2 + row * p.ldr2 + obase;
-        if (EPI == EPI_TRANS && has_bias && valid) row_bias = __ldg(p.bias + row);
+      if (valid) {
+        if (has_fb) fb = p.fbias + static_cast<long long>(static_cast<int>(row) / p.rows_per_frame) * p.ldfb + nbase;
+        if (has_r1) r1p = p.R1 + row * p.ldr1 + obase;
+        if (has_r2) r2p = p.R2 + row * p.ldr2 + obase;
+        if (EPI == EPI_TRANS && has_bias) row_bias = __ldg(p.bias + row);
       }
-      if (has_r1 || has_r2) {
-        // pull the residual row segments of the tile after next into L2 now (two tile-times of lead: these rows
-        // come from HBM); the first iteration also covers the next tile
-        auto prefetch_tile = [&](const TileWalk& w, int cb) {
-          int u0, u1, u2;
-          tile_origin<CONV>(p, w.m_tile * NCTA + cta_rank, u0, u1, u2);
-          long long nrow;
-          if (map_row(u0, u1, u2, nrow)) {
-            const int ncol0 = w.n_tile * OUT_COLS + cb * 16;
+      const uint32_t swz = SUBW == 32 ? static_cast<uint32_t>((tr >> 1) & 3) : 0u;  // 64B-swizzle XOR of the chunk
 #pragma unroll
-            for (int off = 0; off < CH_HALF * 16; off += 64) {
-              if (has_r1) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.R1 + nrow * p.ldr1 + ncol0 + off));
-              if (has_r2) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.R2 + nrow * p.ldr2 + ncol0 + off));
+      for (int j = 0; j < OUT_COLS / 8; ++j) {
+        const int oc = 8 * j + cq;
+        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        if (EPI == EPI_TRANS) {
+          v0 += row_bias;
+          v1 += row_bias;
+        } else if (has_bias) {
+          v0 += __ldg(p.bias + nbase + oc);
+          v1 += __ldg(p.bias + nbase + oc + 1);
+        }
+        if (fb) {
+          v0 += __ldg(fb + oc);
+          v1 += __ldg(fb + oc + 1);
+        }
+        if (GEGLU) {
+          constexpr int JG = BN / 16;  // the gate of column c is column c + BN / 2 of the packed tile
+          float g0 = acc[4 * (j + JG) + 2 * h], g1 = acc[4 * (j + JG) + 2 * h + 1];
+          if (has_bias) {
+            g0 += __ldg(p.bias + nbase + BN / 2 + oc);
+            g1 += __ldg(p.bias + nbase + BN / 2 + oc + 1);
+          }
+          v0 *= gelu_erf_fast(g0);
+          v1 *= gelu_erf_fast(g1);
+        } else if (EPI == EPI_F32 && do_silu) {
+          v0 = silu_f(v0);
+          v1 = silu_f(v1);
+        }
+        if (r1p || r2p) {
+          if (r1p) {
+            const float2 x = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(r1p + oc)));
+            v0 = fmaf(v0, s0, x.x * s1);
+            v1 = fmaf(v1, s0, x.y * s1);
+          } else {
+            v0 *= s0;
+            v1 *= s0;
+          }
+          if (r2p) {
+            const float2 x = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(r2p + oc)));
+            v0 = fmaf(x.x, s2, v0);
+            v1 = fmaf(x.y, s2, v1);
+          }
+        } else if (s0 != 1.0f) {
+          v0 *= s0;
+          v1 *= s0;
+        }
+        if (EPI == EPI_TRANS) {
+          if (valid) {
+            float* dp = static_cast<float*>(p.D) + row;
+            if (obase + oc < p.valid_cols) {
+              float* o = dp + static_cast<long long>(obase + oc) * p.ldd;
+              *o = p.accumulate ? *o + v0 : v0;
+            }
+            if (obase + oc + 1 < p.valid_cols) {
+              float* o = dp + static_cast<long long>(obase + oc + 1) * p.ldd;
+              *o = p.accumulate ? *o + v1 : v1;
             }
           }
-        };
-        const int step = static_cast<int>(gridDim.x) / NCTA;
-        if (iter == 0 && tile + step < total_tiles) prefetch_tile(tw, c_begin_next);
-        if (tile + 2 * step < total_tiles) {
-          TileWalk tw2 = tw;
-          tw2.next();
-          prefetch_tile(tw2, c_begin);
+        } else if (EPI == EPI_F32) {
+          if (valid)
+            *reinterpret_cast<float2*>(static_cast<float*>(p.D) + row * p.ldd + obase + oc) = make_float2(v0, v1);
+        } else {
+          const int sub = oc / SUBW;
+          const int cc = oc - sub * SUBW;
+          const uint32_t addr = stg + static_cast<uint32_t>(sub * C::SUB_BYTES + tr * SUBW * 2) +
+                                ((static_cast<uint32_t>(cc >> 3) ^ swz) << 4) + static_cast<uint32_t>((cc & 7) * 2);
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_bf16x2(v0, v1)) : "memory");
         }
-      }
-
-      // residuals travel one load group ahead: group g+1's rows are requested before group g is processed, so they
-      // have landed by the time the proxy fence (a full CTA memory barrier) of group g is reached
-      uint4 na[LG][2];
-#pragma unroll
-      for (int hh = 0; hh < LG; ++hh) na[hh][0] = na[hh][1] = make_uint4(0, 0, 0, 0);
-      auto load_res = [&](int g) {
-        if (RTMA) return;  // the residual sub-tiles arrive through TMA (below)
-#pragma unroll
-        for (int hh = 0; hh < LG; ++hh) {
-          const int c = (c_begin + g * LG + hh) * 16;
-          if (r1p) { na[hh][0] = __ldg(reinterpret_cast<const uint4*>(r1p + c)); na[hh][1] = __ldg(reinterpret_cast<const uint4*>(r1p + c) + 1); }
-        }
-      };
-      // RTMA: the group's store leader requests residual sub-tile `sub` (index within this tile's share) into the
-      // buffer the sub-tile counter selects; the TMA clips at row / image tails like the output store (zero fill)
-      auto request_res = [&](int col0, int o0, int o1, int o2, uint32_t slot) {
-        const uint32_t sl = slot % RD;
-        uint8_t* dst = rbuf + sl * SUB_BYTES;
-        mbar_arrive_expect_tx(&rfull[sl], SUB_BYTES);
-        if (CONV) tma_load_4d(dst, &mapR, &rfull[sl], col0, o0, o1, o2);
-        else tma_load_3d(dst, &mapR, &rfull[sl], col0, o1, o0);
-      };
-      // the first RD sub-tiles of a tile are requested at the end of the previous tile (below); only the very first
-      // tile of this CTA requests its own
-      if (RTMA && store_leader && iter == 0) {
-#pragma unroll
-        for (uint32_t j = 0; j < RD; ++j)
-          if (static_cast<int>(j) * LG < my_n)
-            request_res(obase + (c_begin + static_cast<int>(j) * LG) * 16, t0, t1, t2, nstore + j);
-      }
-      if (my_n > 0) load_res(0);
-#pragma unroll
-      for (int g = 0; g < NG_HALF; ++g) {
-        if (g * LG < my_n) {
-          tmem_ld_wait();
-          V3D_ETRACE();  // group: TMEM data landed
-          if ((g + 1) * LG < my_n) issue_group(g + 1, vb[(g + 1) & 1]);
-          uint4 ca[LG][2], cb[LG][2];
-          if (RTMA) mbar_wait(&rfull[nstore % RD], (nstore / RD) & 1u);  // this sub-tile's residual rows have landed
-#pragma unroll
-          for (int hh = 0; hh < LG; ++hh) {
-            if (RTMA) {
-              const uint32_t rrow = smem_u32(rbuf) + (nstore % RD) * SUB_BYTES + row_off;
-              ca[hh][0] = lds128(rrow + (((hh * 2) ^ swz) << 4));
-              ca[hh][1] = lds128(rrow + (((hh * 2 + 1) ^ swz) << 4));
-            } else {
-              ca[hh][0] = na[hh][0];
-              ca[hh][1] = na[hh][1];
-            }
-            cb[hh][0] = cb[hh][1] = make_uint4(0, 0, 0, 0);
-            // the second residual (blend epilogue only) is fetched for the current group: its rows were pulled
-            // into L2 two tiles ago, and holding a second prefetched set would spill
-            if (r2p) {
-              const int c = (c_begin + g * LG + hh) * 16;
-              cb[hh][0] = __ldg(reinterpret_cast<const uint4*>(r2p + c));
-              cb[hh][1] = __ldg(reinterpret_cast<const uint4*>(r2p + c) + 1);
-            }
-          }
-          if ((g + 1) * LG < my_n) load_res(g + 1);
-#pragma unroll
-          for (int hh = 0; hh < LG; ++hh) {
-            const int k = g * LG + hh;
-            const int c = (c_begin + k) * 16;
-            const uint32_t* v = &vb[g & 1][GEGLU ? 0 : hh * 16];
-            const uint32_t* gv = &vb[g & 1][GEGLU ? 16 : 0];
-            const uint4 ra0 = ca[hh][0], ra1 = ca[hh][1], rb0 = cb[hh][0], rb1 = cb[hh][1];
-            // all epilogue arithmetic runs on packed f32x2 pairs (FADD2 / FMUL2 / FFMA2: half the issue slots)
-            uint64_t f2[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) f2[j] = pack2(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1]));
-            // bias vectors are shared by every row: after the first warp touched them they are L1 hits
-            if (EPI == EPI_TRANS) {
-              const uint64_t rb2 = pack2(row_bias, row_bias);
-#pragma unroll
-              for (int j = 0; j < 8; ++j) f2[j] = add2(f2[j], rb2);
-            } else if (has_bias || (has_fb && p.fb_uniform)) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const float b0 = __shfl_sync(0xffffffffu, breg[(k * 16 + 2 * j) >> 5], (k * 16 + 2 * j) & 31);
-                const float b1 = __shfl_sync(0xffffffffu, breg[(k * 16 + 2 * j + 1) >> 5], (k * 16 + 2 * j + 1) & 31);
-                f2[j] = add2(f2[j], pack2(b0, b1));
-              }
-            }
-            if (fb) {
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const float4 b4 = __ldg(reinterpret_cast<const float4*>(fb + c) + j);
-                f2[2 * j] = add2(f2[2 * j], pack2(b4.x, b4.y));
-                f2[2 * j + 1] = add2(f2[2 * j + 1], pack2(b4.z, b4.w));
-              }
-            }
-            if (GEGLU) {
-              uint64_t g2[8];
-#pragma unroll
-              for (int j = 0; j < 8; ++j) g2[j] = pack2(__uint_as_float(gv[2 * j]), __uint_as_float(gv[2 * j + 1]));
-              if (has_bias) {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  const float b0 = __shfl_sync(0xffffffffu, greg[(k * 16 + 2 * j) >> 5], (k * 16 + 2 * j) & 31);
-                  const float b1 = __shfl_sync(0xffffffffu, greg[(k * 16 + 2 * j + 1) >> 5], (k * 16 + 2 * j + 1) & 31);
-                  g2[j] = add2(g2[j], pack2(b0, b1));
-                }
-              }
-#pragma unroll
-              for (int j = 0; j < 8; ++j) f2[j] = mul2(f2[j], gelu_erf_fast2(g2[j]));
-            } else if (EPI == EPI_F32 && do_silu) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                float a, b;
-                unpack2(f2[j], a, b);
-                f2[j] = pack2(silu_f(a), silu_f(b));
-              }
-            }
-            if (r1p || r2p) {
-              const uint64_t s0v = pack2(s0, s0), s1v = pack2(s1, s1), s2v = pack2(s2, s2);
-              if (r1p) {
-                const uint32_t u[8] = {ra0.x, ra0.y, ra0.z, ra0.w, ra1.x, ra1.y, ra1.z, ra1.w};
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  const float2 x2 = unpack_bf16x2(u[j]);
-                  f2[j] = fma2(f2[j], s0v, mul2(pack2(x2.x, x2.y), s1v));
-                }
-              } else {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) f2[j] = mul2(f2[j], s0v);
-              }
-              if (r2p) {
-                const uint32_t u[8] = {rb0.x, rb0.y, rb0.z, rb0.w, rb1.x, rb1.y, rb1.z, rb1.w};
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  const float2 x2 = unpack_bf16x2(u[j]);
-                  f2[j] = fma2(pack2(x2.x, x2.y), s2v, f2[j]);
-                }
-              }
-            } else if (s0 != 1.0f) {
-              const uint64_t s0v = pack2(s0, s0);
-#pragma unroll
-              for (int j = 0; j < 8; ++j) f2[j] = mul2(f2[j], s0v);
-            }
-            float f[16];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) unpack2(f2[j], f[2 * j], f[2 * j + 1]);
-            if (EPI == EPI_TRANS) {
-              // D[col][row]: lanes hold consecutive rows -> each store instruction is one contiguous 128-byte line
-              if (valid) {
-                float* dp = static_cast<float*>(p.D) + row;
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                  if (obase + c + j < p.valid_cols) {
-                    float* o = dp + static_cast<long long>(obase + c + j) * p.ldd;
-                    *o = p.accumulate ? *o + f[j] : f[j];
-                  }
-                }
-              }
-            } else if (EPI == EPI_F32) {
-              if (valid) {
-                float4* dp = reinterpret_cast<float4*>(static_cast<float*>(p.D) + row * p.ldd + obase + c);
-#pragma unroll
-                for (int j = 0; j < 4; ++j) dp[j] = make_float4(f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]);
-              }
-            } else if (!V3D_DBG(1)) {
-              // bf16 rows leave through TMA.  The chunk goes into this row's slot of the group's current buffer
-              // (64-byte rows, 64B-swizzled: conflict-free 16-byte stores); when the sub-tile is complete the
-              // group meets on its named barrier and one thread issues the 128-row store, which the hardware
-              // clips at the tensor edge (row tails, image tails).
-              const uint32_t buf = stg + static_cast<uint32_t>((nstore & 1) * SUB_BYTES) + row_off;
-              const int part = k % CPS;
-              if (!V3D_DBG(32)) {
-                sts128(buf + (((part * 2) ^ swz) << 4), pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]),
-                       pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
-                sts128(buf + (((part * 2 + 1) ^ swz) << 4), pack_bf16x2(f[8], f[9]), pack_bf16x2(f[10], f[11]),
-                       pack_bf16x2(f[12], f[13]), pack_bf16x2(f[14], f[15]));
-              }
-              if (part == CPS - 1) {
-                if (!V3D_DBG(16)) fence_proxy_async_smem();
-                V3D_ETRACE();  // sub-tile rows written + fenced
-                // the previous store (other buffer) must have drained before anyone refills it after the barrier
-                if (store_leader && !V3D_DBG(8)) bulk_wait_read<0>();
-                V3D_ETRACE();  // previous store drained
-                asm volatile("bar.sync %0, 128;" ::"r"(1 + half) : "memory");
-                V3D_ETRACE();  // group met
-                if (store_leader && !V3D_DBG(2)) {
-                  const uint32_t src = stg + static_cast<uint32_t>((nstore & 1) * SUB_BYTES);
-                  const int col0 = obase + c - (CPS - 1) * 16;
-                  if (CONV) tma_store_4d(&mapD, src, col0, t0, t1, t2);
-                  else tma_store_3d(&mapD, src, col0, t1, t0);
-                  if (!CONV && EPI == EPI_BF16 && kv.n > 0 && col0 >= kv.col0) {
-                    // fused all-gather: the same sub-tile into every rank's gather buffer (peer memory over NVLink)
-                    for (int i = 0; i < kv.n; ++i) tma_store_3d(&kv.m[i], src, col0 - kv.col0, t1, t0);
-                  }
-                  bulk_commit();
-                }
-                V3D_ETRACE();  // sub-tile handed to TMA
-                // RTMA: every thread of the group read this sub-tile's residual slot before the barrier above, so
-                // the slot can take the sub-tile RD further on
-                if (RTMA && store_leader && (g + static_cast<int>(RD)) * LG < my_n)
-                  request_res(obase + (c_begin + (g + static_cast<int>(RD)) * LG) * 16, t0, t1, t2, nstore);
-                ++nstore;
-              }
-            }
-          }
-        }
-      }
-      if (RTMA && store_leader && tile + static_cast<int>(gridDim.x) / NCTA < total_tiles) {
-        // every residual slot is free now (every thread of the group passed the last sub-tile's barrier): request
-        // the head of the NEXT tile's share, so that it is in shared memory before that tile's accumulator is ready
-        int u0, u1, u2;
-        tile_origin<CONV>(p, tw.m_tile * NCTA + cta_rank, u0, u1, u2);
-        const int hsel_next = (NSUB & 1) ? (half ^ ((iter + 1) & 1)) : half;
-        const int my_n_next = hsel_next ? NCH - CH_HALF : CH_HALF;
-        const int col_next = tw.n_tile * OUT_COLS + c_begin_next * 16;
-#pragma unroll
-        for (uint32_t j = 0; j < RD; ++j)
-          if (static_cast<int>(j) * LG < my_n_next)
-            request_res(col_next + static_cast<int>(j) * LG * 16, u0, u1, u2, nstore + j);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (NCTA == 2) mbar_arrive_leader(&tempty_bar[acc]);
-        else mbar_arrive(&tempty_bar[acc]);
-      }
-      V3D_ETRACE();  // tile done
-      if (++acc == C::ACC_STAGES) {
-        acc = 0;
-        acc_phase ^= 1u;
       }
     }
-#undef V3D_ETRACE
-    if (STAGED && lane == 0) bulk_wait_all();  // smem slabs must outlive the last TMA store reads
+    if (C::STAGED) {
+      // the whole bf16 tile is in shared memory: one thread hands it to TMA, which clips at row / image tails
+      fence_proxy_async_smem();
+      asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory");
+      if (store_leader) {
+#pragma unroll 1
+        for (int sub = 0; sub < C::NSUB; ++sub) {
+          const uint32_t src = stg + static_cast<uint32_t>(sub * C::SUB_BYTES);
+          const int col0 = obase + sub * SUBW;
+          if (CONV) tma_store_4d(&mapD, src, col0, t0, t1, t2);
+          else tma_store_3d(&mapD, src, col0, t1, t0);
+          if (!CONV && EPI == EPI_BF16 && kv.n > 0 && col0 >= kv.col0) {
+            // fused all-gather: the same sub-tile into every rank's gather buffer (peer memory over NVLink)
+            for (int i = 0; i < kv.n; ++i) tma_store_3d(&kv.m[i], src, col0 - kv.col0, t1, t0);
+          }
+        }
+        bulk_commit();
+      }
+    }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (NCTA == 2) cluster_sync_all();  // the peer's shared memory and TMEM stay alive until the leader's MMAs retired
-  if (warp == 1) {
-    tc_fence_after();
-    if (NCTA == 2) tmem_dealloc_2cta(tmem_base, C::TMEM_COLS);
-    else tmem_dealloc(tmem_base, C::TMEM_COLS);
-  }
+  if (C::STAGED && store_leader) bulk_wait_all();  // the staging buffer must outlive the last TMA store reads
 }
 
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-static long long* g_trace = nullptr;  // diagnostics: set through v3d_debug_set_trace
 static int pick_block_n(int N, int act) {
   static const int cands[] = {256, 160, 128, 64, 32, 16};
   for (int c : cands) {
@@ -733,13 +398,12 @@ static int pick_block_n(int N, int act) {
 static KvMaps g_kv_none;  // zero-initialised: n = 0
 static const KvMaps* g_kv = &g_kv_none;  // set by v3d_gemm_bf16 around the one launch that scatters K|V
 
-template <int BN, bool CONV, int EPI, int NCTA = 1>
+template <int BN, bool CONV, int EPI>
 static int launch(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& md, const GemmEpi& epi,
-                  cudaStream_t st, const CUtensorMap* mr = nullptr) {
-  using C = Cfg<BN, NCTA, EPI == EPI_BF16RT>;
-  const CUtensorMap& mres = mr ? *mr : md;  // only the EPI_BF16RT instantiations read it
+                  cudaStream_t st) {
+  using C = Cfg<BN, EPI>;
   static bool configured = false;
-  auto kern = gemm_tc_kernel<BN, CONV, EPI, NCTA>;
+  auto kern = gemm_tc_kernel<BN, CONV, EPI>;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
     if (e != cudaSuccess) {
@@ -748,72 +412,25 @@ static int launch(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMa
     }
     configured = true;
   }
-  if (NCTA == 1) {
-    const int total = epi.num_m_tiles * epi.num_n_tiles;
-    const int grid = total < num_sms() ? total : num_sms();
-    kern<<<grid, kThreads, C::SMEM_BYTES, st>>>(ma, mb, md, epi, mres, *g_kv);
-  } else {
-    // one cluster of two CTAs per 256-row pair tile, persistent over at most num_sms / 2 clusters
-    const int total = ((epi.num_m_tiles + 1) / 2) * epi.num_n_tiles;
-    const int clusters = total < num_sms() / 2 ? total : num_sms() / 2;
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(static_cast<unsigned>(2 * clusters));
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = C::SMEM_BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ma, mb, md, epi, mres, *g_kv);
-    if (e != cudaSuccess) {
-      set_error("gemm_tc_kernel (CTA pair) launch failed: %s", cudaGetErrorString(e));
-      return V3D_ERR_CUDA;
-    }
-  }
+  const int total = epi.num_m_tiles * epi.num_n_tiles;
+  const int grid = total < num_sms() ? total : num_sms();
+  kern<<<grid, kThreads, C::SMEM_BYTES, st>>>(ma, mb, md, epi, *g_kv);
   V3D_CHECK_LAUNCH("gemm_tc_kernel");
   return V3D_OK;
 }
 
-// CTA-pair variants exist for the wide bf16-output tiles only (the shapes that are ingest- or shared-memory-bound
-// with one CTA: 160-wide UNet layers, the 128-wide decoder levels)
-template <int BN, bool CONV>
-static int dispatch_epi_pair(int epi_kind, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& md,
-                             const GemmEpi& epi, cudaStream_t st) {
-  if constexpr (BN == 128 || BN == 160 || BN == 256) {
-    switch (epi_kind) {
-      case EPI_BF16: return launch<BN, CONV, EPI_BF16, 2>(ma, mb, md, epi, st);
-      case EPI_BF16R2: return launch<BN, CONV, EPI_BF16R2, 2>(ma, mb, md, epi, st);
-      case EPI_GEGLU:
-        if constexpr (!CONV && BN == 256) return launch<256, false, EPI_GEGLU, 2>(ma, mb, md, epi, st);
-        break;
-    }
-  }
-  set_error("no CTA-pair variant for epilogue %d / block_n %d", epi_kind, BN);
-  return V3D_ERR_BAD_ARG;
-}
-
 template <int BN, bool CONV>
 static int dispatch_epi(int epi_kind, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& md,
-                        const GemmEpi& epi, cudaStream_t st, const CUtensorMap* mr = nullptr) {
+                        const GemmEpi& epi, cudaStream_t st) {
   switch (epi_kind) {
     case EPI_BF16: return launch<BN, CONV, EPI_BF16>(ma, mb, md, epi, st);
-    case EPI_BF16RT:
-      if constexpr (BN % 32 == 0 && BN >= 64) {
-        if (mr != nullptr) return launch<BN, CONV, EPI_BF16RT>(ma, mb, md, epi, st, mr);
-      }
-      break;
     case EPI_BF16R2: return launch<BN, CONV, EPI_BF16R2>(ma, mb, md, epi, st);
     case EPI_F32: return launch<BN, CONV, EPI_F32>(ma, mb, md, epi, st);
     case EPI_GEGLU:
       if constexpr (!CONV && (BN / 2) % 16 == 0) return launch<BN, false, EPI_GEGLU>(ma, mb, md, epi, st);
       break;
-    case EPI_TRANS:
-      if constexpr (!CONV) return launch<BN, false, EPI_TRANS>(ma, mb, md, epi, st);
+    case EPI_TRANS:  // at most 128 columns: the per-element transposed stores of wider tiles spill (host caps bn)
+      if constexpr (!CONV && BN <= 128) return launch<BN, false, EPI_TRANS>(ma, mb, md, epi, st);
       break;
   }
   set_error("unsupported epilogue %d for this mode/tile", epi_kind);
@@ -822,22 +439,14 @@ static int dispatch_epi(int epi_kind, const CUtensorMap& ma, const CUtensorMap& 
 
 template <bool CONV>
 static int dispatch_bn(int bn, int epi_kind, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& md,
-                       const GemmEpi& epi, cudaStream_t st, bool pair = false, const CUtensorMap* mr = nullptr) {
-  if (pair) {
-    switch (bn) {
-      case 256: return dispatch_epi_pair<256, CONV>(epi_kind, ma, mb, md, epi, st);
-      case 160: return dispatch_epi_pair<160, CONV>(epi_kind, ma, mb, md, epi, st);
-      case 128: return dispatch_epi_pair<128, CONV>(epi_kind, ma, mb, md, epi, st);
-      default: set_error("no CTA-pair variant for block_n %d", bn); return V3D_ERR_BAD_ARG;
-    }
-  }
+                       const GemmEpi& epi, cudaStream_t st) {
   switch (bn) {
-    case 256: return dispatch_epi<256, CONV>(epi_kind, ma, mb, md, epi, st, mr);
-    case 160: return dispatch_epi<160, CONV>(epi_kind, ma, mb, md, epi, st, mr);
-    case 128: return dispatch_epi<128, CONV>(epi_kind, ma, mb, md, epi, st, mr);
-    case 64: return dispatch_epi<64, CONV>(epi_kind, ma, mb, md, epi, st, mr);
-    case 32: return dispatch_epi<32, CONV>(epi_kind, ma, mb, md, epi, st, mr);
-    case 16: return dispatch_epi<16, CONV>(epi_kind, ma, mb, md, epi, st, mr);
+    case 256: return dispatch_epi<256, CONV>(epi_kind, ma, mb, md, epi, st);
+    case 160: return dispatch_epi<160, CONV>(epi_kind, ma, mb, md, epi, st);
+    case 128: return dispatch_epi<128, CONV>(epi_kind, ma, mb, md, epi, st);
+    case 64: return dispatch_epi<64, CONV>(epi_kind, ma, mb, md, epi, st);
+    case 32: return dispatch_epi<32, CONV>(epi_kind, ma, mb, md, epi, st);
+    case 16: return dispatch_epi<16, CONV>(epi_kind, ma, mb, md, epi, st);
     default: set_error("unsupported block_n %d", bn); return V3D_ERR_BAD_ARG;
   }
 }
@@ -846,20 +455,14 @@ static int dispatch_bn(int bn, int epi_kind, const CUtensorMap& ma, const CUtens
 
 using namespace v3d;
 
-/* diagnostics: device buffer of >= 3072 int64 that CTA 0 of every subsequent GEMM launch fills with clock64()
- * timelines (producer k-blocks | MMA issuer | epilogue warp 2); NULL disables. Not part of the product path. */
+/* diagnostics hook of an earlier GEMM (per-role clock64 timelines); this kernel records none: NULL is accepted,
+ * anything else is refused. */
 extern "C" int v3d_debug_set_trace(void* buf) {
-#ifdef V3D_GEMM_DIAG
-  g_trace = static_cast<long long*>(buf);
-  return V3D_OK;
-#else
   if (buf != nullptr) {
-    set_error("v3d_debug_set_trace: library built without V3D_GEMM_DIAG");
+    set_error("v3d_debug_set_trace: the GEMM records no role timelines");
     return V3D_ERR_UNSUPPORTED;
   }
-  g_trace = nullptr;
   return V3D_OK;
-#endif
 }
 
 extern "C" int v3d_gemm_pick_block_n(int32_t N, int32_t act) { return pick_block_n(N, act); }
@@ -939,6 +542,14 @@ extern "C" int v3d_gemm_bf16(const v3d_gemm_args* a, void* stream) {
       }
     }
   }
+  if (a->out_transposed && a->block_n <= 0 && bn > 128) {  // the transposed fp32 epilogue exists up to 128 columns
+    for (int c : {128, 64, 32, 16}) {
+      if (a->N % c == 0) {
+        bn = c;
+        break;
+      }
+    }
+  }
   if (bn == 0 || a->N % bn != 0 || (a->act == V3D_ACT_GEGLU && (bn / 2) % 16 != 0)) {
     set_error("v3d_gemm_bf16: no valid N tile for N=%d act=%d block_n=%d", a->N, a->act, a->block_n);
     return V3D_ERR_BAD_ARG;
@@ -963,25 +574,6 @@ extern "C" int v3d_gemm_bf16(const v3d_gemm_args* a, void* stream) {
   e.rows_per_frame = a->rows_per_frame > 0 ? a->rows_per_frame : 1;
   e.act = a->act;
   e.out_fp32 = a->out_fp32;
-  {
-    static int dbg = -1;
-    if (dbg < 0) {
-      const char* v = getenv("V3D_GEMM_DEBUG");
-      dbg = v ? atoi(v) : 0;
-    }
-    e.dbg = dbg;
-    e.trace = g_trace;
-  }
-  if (a->fbias != nullptr) {
-    if (conv) {
-      const int bw_ = a->conv_w < BM ? a->conv_w : BM;
-      int bh_ = BM / bw_;
-      if (bh_ > a->conv_h) bh_ = a->conv_h;
-      e.fb_uniform = (bw_ * bh_) % 32 == 0 && e.rows_per_frame % (a->conv_w * a->conv_h) == 0;
-    } else {
-      e.fb_uniform = e.rows_per_frame % 32 == 0 && (a->batch <= 1 || a->rows_per_batch % 32 == 0);
-    }
-  }
   e.transposed = a->out_transposed;
   e.valid_cols = a->valid_cols > 0 ? a->valid_cols : a->N;
   e.accumulate = a->accumulate;
@@ -1065,34 +657,12 @@ extern "C" int v3d_gemm_bf16(const v3d_gemm_args* a, void* stream) {
       e.b_batched = 1;
     }
   }
-  // CTA-pair (cta_group::2) tiles, wide bf16-output tiles only.  V3D_GEMM_2CTA: unset / "auto" = per-shape choice
-  // from the round-2 hardware timings (profiles/microbench_r2_pair_rtma.md: +5..8 % on the 256-wide GEGLU and decoder
-  // conv tiles, +12 % on the decoder's 128-wide top level, +2..3 % on the residual-free projections; temporal convs,
-  // residual epilogues and short grids lose), "1" = every eligible tile, "0" = never.
-  bool pair = false;
-  {
-    static int want_pair = -2;
-    if (want_pair == -2) {
-      const char* v = getenv("V3D_GEMM_2CTA");
-      want_pair = (v == nullptr || v[0] == 'a') ? -1 : (atoi(v) != 0 ? 1 : 0);
-    }
-    const bool staged_out = !a->out_transposed && !a->out_fp32;
-    const bool eligible = staged_out && e.num_m_tiles >= 2 &&
-                          (bn == 256 || ((bn == 160 || bn == 128) && a->act != V3D_ACT_GEGLU));
-    if (want_pair == 1) {
-      pair = eligible;
-    } else if (want_pair == -1 && eligible && a->R1 == nullptr && a->R2 == nullptr) {
-      if (a->act == V3D_ACT_GEGLU) pair = e.num_m_tiles >= 16;
-      else if (conv) pair = e.num_m_tiles >= 64 && (bn != 160 || a->K >= 640);
-      else if (ntaps == 1) pair = e.num_m_tiles >= 64 && b_batch == 1;
-    }
-  }
   {
     const uint64_t ktot = (uint64_t)ntaps * a->K;
     const uint64_t bbs = b_batch > 1 ? (uint64_t)a->b_batch_stride : (uint64_t)a->N * a->ldb;
     const uint64_t dims[3] = {ktot, (uint64_t)a->N, (uint64_t)b_batch};
     const uint64_t str[2] = {(uint64_t)a->ldb * 2, bbs * 2};
-    const uint32_t box[3] = {BK, (uint32_t)(pair ? bn / 2 : bn), 1};  // a pair stages half of the B tile per CTA
+    const uint32_t box[3] = {BK, (uint32_t)bn, 1};
     rc = make_tmap_bf16(&mb, a->B, 3, dims, str, box);
     if (rc) return rc;
   }
@@ -1112,24 +682,7 @@ extern "C" int v3d_gemm_bf16(const v3d_gemm_args* a, void* stream) {
     e.R2 = nullptr;
   }
   if (epi_kind == EPI_BF16 && e.R2 != nullptr) epi_kind = EPI_BF16R2;
-  // TMA-staged residual (EPI_BF16RT): single residual, 32-column sub-tiles, one CTA.  V3D_GEMM_RTMA: unset / "auto" =
-  // the short-K linear projections (K <= 640: +30 % at K = 320, +10 % at K = 640 on hardware; longer K loses a pipeline
-  // stage to the residual ring and gets slower), "1" = every eligible launch, "0" = never.
-  bool rtma = false;
-  {
-    static int want_rtma = -2;
-    if (want_rtma == -2) {
-      const char* v = getenv("V3D_GEMM_RTMA");
-      want_rtma = (v == nullptr || v[0] == 'a') ? -1 : (atoi(v) != 0 ? 1 : 0);
-    }
-    const bool eligible = epi_kind == EPI_BF16 && e.R1 != nullptr && !pair && bn % 32 == 0 && bn >= 64 &&
-                          (reinterpret_cast<uintptr_t>(e.R1) & 15u) == 0;
-    rtma = eligible && (want_rtma == 1 || (want_rtma == -1 && !conv && ntaps == 1 && a->K <= 640 && e.num_m_tiles >= 64));
-  }
-  if (rtma) epi_kind = EPI_BF16RT;
-  CUtensorMap mr;
-  memset(&mr, 0, sizeof(mr));
-  if (epi_kind == EPI_BF16 || epi_kind == EPI_BF16R2 || epi_kind == EPI_GEGLU || epi_kind == EPI_BF16RT) {
+  if (epi_kind == EPI_BF16 || epi_kind == EPI_BF16R2 || epi_kind == EPI_GEGLU) {
     const uint64_t out_cols = static_cast<uint64_t>(e.num_n_tiles) * (epi_kind == EPI_GEGLU ? bn / 2 : bn);
     const uint32_t ocols_tile = epi_kind == EPI_GEGLU ? bn / 2 : bn;
     const uint32_t subw = ocols_tile % 32 == 0 ? 32 : 16;  // must match SUBW in the kernel
@@ -1146,20 +699,6 @@ extern "C" int v3d_gemm_bf16(const v3d_gemm_args* a, void* stream) {
       rc = make_tmap_bf16(&md, a->D, 3, dims, str, box, swz);
     }
     if (rc) return rc;
-    if (rtma) {  // the residual through the same geometry as the output: [cols][rows...] with row stride ldr1
-      if (conv) {
-        const uint64_t dims[4] = {out_cols, (uint64_t)e.cw, (uint64_t)e.ch, (uint64_t)e.cn};
-        const uint64_t str[3] = {(uint64_t)e.ldr1 * 2, (uint64_t)e.ldr1 * 2 * e.cw, (uint64_t)e.ldr1 * 2 * e.cw * e.ch};
-        const uint32_t box[4] = {subw, (uint32_t)e.bw, (uint32_t)e.bh, (uint32_t)e.bn};
-        rc = make_tmap_bf16(&mr, e.R1, 4, dims, str, box, swz);
-      } else {
-        const uint64_t dims[3] = {out_cols, (uint64_t)e.rows_per_batch, (uint64_t)e.batch};
-        const uint64_t str[2] = {(uint64_t)e.ldr1 * 2, (uint64_t)e.ldr1 * 2 * e.rows_per_batch};
-        const uint32_t box[3] = {subw, BM, 1};
-        rc = make_tmap_bf16(&mr, e.R1, 3, dims, str, box, swz);
-      }
-      if (rc) return rc;
-    }
   }
   // fused GEMM -> all-gather (K|V scatter into peer memory): plain linear bf16-output launches only
   KvMaps kvm;
@@ -1186,8 +725,7 @@ extern "C" int v3d_gemm_bf16(const v3d_gemm_args* a, void* stream) {
     }
     g_kv = &kvm;
   }
-  rc = conv ? dispatch_bn<true>(bn, epi_kind, ma, mb, md, e, st, pair, rtma ? &mr : nullptr)
-            : dispatch_bn<false>(bn, epi_kind, ma, mb, md, e, st, pair, rtma ? &mr : nullptr);
+  rc = conv ? dispatch_bn<true>(bn, epi_kind, ma, mb, md, e, st) : dispatch_bn<false>(bn, epi_kind, ma, mb, md, e, st);
   g_kv = &g_kv_none;
   return rc;
 }

@@ -176,6 +176,10 @@ int v3d_peer_alloc(int64_t bytes, void** out) {
   void* p = nullptr;
   cudaError_t e = cudaMalloc(&p, static_cast<size_t>(bytes));
   if (e == cudaSuccess) e = cudaMemset(p, 0, static_cast<size_t>(bytes));
+  // the zeroing must have landed before the handle can be exported: cudaMemset only enqueues it behind this process's
+  // pending work, and a peer that already holds the handle may write data and epoch flags into the arena at once; a
+  // memset that runs after those writes would erase them and leave the owner waiting for a signal that never comes
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
   if (e != cudaSuccess) {
     set_error("v3d_peer_alloc(%lld): %s", static_cast<long long>(bytes), cudaGetErrorString(e));
     if (p) cudaFree(p);

@@ -1,4 +1,4 @@
-"""B200-native first-stage decode: drop-ins for `sgm.modules.autoencoding.temporal_ae.VideoDecoder`
+"""H100-native first-stage decode: drop-ins for `sgm.modules.autoencoding.temporal_ae.VideoDecoder`
 (temporal_ae.py:293-349 over diffusionmodules/model.py:604-748) and the decode side of
 `sgm.models.autoencoder.AutoencodingEngine` (autoencoder.py:196-212).
 

@@ -1,4 +1,4 @@
-"""B200-native first-stage ENCODE front-end (SURVEY.md 8(f) rank 1): drop-in for
+"""H100-native first-stage ENCODE front-end (SURVEY.md 8(f) rank 1): drop-in for
 `sgm.modules.diffusionmodules.model.Encoder` (model.py:463-601, config configs/ae/video.yaml) and the Gaussian
 posterior of `DiagonalGaussianRegularizer` (regularizers/__init__.py:13-32, distributions.py:24-41).
 
@@ -9,7 +9,7 @@ keys as the reference encoder; forward takes NCHW fp32 images in [-1, 1] and ret
 [B, 2*z, H/8, W/8].
 
 Oracle restatement pinned against the real reference, golden fixtures under tests/golden/encoder_*; the device path is
-checked against them in tests/test_parity_gpu.py::test_encoder_matches_reference (green on B200).
+checked against them in tests/test_parity_gpu.py::test_encoder_matches_reference.
 """
 from __future__ import annotations
 

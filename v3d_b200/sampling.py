@@ -175,7 +175,7 @@ class Denoiser(nn.Module):
         super().__init__()
         self.scaling = instantiate_from_config(scaling_config)
         if not isinstance(self.scaling, VScalingWithEDMcNoise):
-            raise NotImplementedError("only VScalingWithEDMcNoise is implemented on the B200 path")
+            raise NotImplementedError("only VScalingWithEDMcNoise is implemented on the native path")
 
     def possibly_quantize_sigma(self, sigma: torch.Tensor) -> torch.Tensor:
         return sigma

@@ -58,6 +58,6 @@ def run(verbose: bool = True) -> dict:
         print("smoke:", res)
     assert launches > 0, "no native kernels were launched"
     assert torch.isfinite(got).all()
-    # the parity tolerance of DESIGN.md section 4 (measured 2.3e-2 / 0.9997 on this composition: sampler + UNet + decode)
+    # the parity tolerance of DESIGN.md section 4 (measured 2.33e-2 / 0.99973 and 2.39e-2 / 0.99972 in two runs on one H100 for this composition: sampler + UNet + decode)
     assert rel <= 3e-2 and cos >= 0.999, f"smoke parity failed: {res}"
     return res

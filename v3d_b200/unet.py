@@ -1,4 +1,4 @@
-"""B200-native drop-in for sgm.modules.diffusionmodules.video_model.VideoUNet (reference
+"""H100-native drop-in for sgm.modules.diffusionmodules.video_model.VideoUNet (reference
 sgm/modules/diffusionmodules/video_model.py:84-493).
 
 Same constructor kwargs, same `state_dict()` keys/shapes (SURVEY.md App. D), same forward signature; the
@@ -187,9 +187,11 @@ class KernelModule(nn.Module):
     def _gn(self, P: dict, key: str, x: torch.Tensor, rows_per_sample: int, nsamples: int, c: int, eps: float,
             silu: bool) -> torch.Tensor:
         y = torch.empty(x.shape[0], c, device=x.device, dtype=torch.bfloat16)
-        # one launch (statistics -> grid barrier -> apply) where it measured faster than the statistics + apply pair:
-        # per-frame (2-D) norms whose tensor can still be re-read from the 126 MB L2 (-13..-23 % at the UNet's shapes);
-        # the 3-D time_stack norms (2 samples) and the decoder's GB-sized tensors stay on the pair
+        # one launch (statistics -> grid barrier -> apply) for the per-frame (2-D) norms: on one H100 it measured faster
+        # than the statistics + apply pair at every such UNet shape (tools/microbench.py norm: 0.116 vs 0.139 ms at
+        # [36*4096, 320], 0.324 vs 0.325 at 960 channels, 0.063 vs 0.091 at level 1, 0.035 vs 0.042 at level 2) and up to
+        # 604 MB tensors (0.641 vs 0.669 ms); the UNet's largest is 283 MB, so the 300 MB bound excludes none of them.
+        # At 1.2 GB the two tie.  The 3-D time_stack norms (2 samples) stay on the pair
         fused = 8 <= nsamples <= 256 and x.numel() * 2 <= 300e6
         if fused and os.environ.get("V3D_GN_FUSED", "1") != "0":
             return ops.groupnorm(x, y, P[key + ".weight"], P[key + ".bias"], rows_per_sample, nsamples, c, eps, silu,
@@ -649,7 +651,7 @@ class VideoUNet(KernelModule):
         assert tuple(ind.shape) == (b, T), f"image_only_indicator must be [{b},{T}], got {tuple(ind.shape)}"
         if bool(ind.bool().any()):
             raise NotImplementedError("image_only_indicator != 0 (image frames mixed into a video batch) is not "
-                                      "implemented in the B200 kernels")
+                                      "implemented in the native kernels")
         self._indicator_seen = tag
 
     def forward(

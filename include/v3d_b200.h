@@ -222,6 +222,37 @@ int v3d_euler_step(const void* x, const void* den, const void* sigma_hat, const 
  * else the Euler proposal; x_euler = euler step of x, den2 = denoised(x_euler, sigma_next). out may alias x. */
 int v3d_heun_step(const void* x, const void* den, const void* x_euler, const void* den2, const void* sigma_hat,
                   const void* sigma_next, void* out, int32_t nsamples, int64_t per_sample, void* stream);
+/* The ancestral, DPM++ and linear-multistep samplers (sampling.py:136-211,240-365; sampling_utils.py:7-43).  One pass
+ * over the fp32 state per call; every sample shares the step's sigma, so the schedule-derived multipliers are host
+ * scalars computed in fp32 like the reference's.  Each operation is rounded on its own, in the reference's order
+ * (e.g. (noise * s_noise) * sigma_up), so the results are the reference's to the last bit.  The noise term is added
+ * only where sigma_next > 0 (ancestral_step's torch.where); the caller still draws that step's noise, as the
+ * reference does, so later draws stay in the reference's order. */
+#define V3D_LMS_MAX_ORDER 8
+/* EulerAncestralSampler step: d = (x - den)/sigma; x_euler = x + (sigma_down - sigma) d; out = sigma_next > 0 ?
+ * x_euler + (noise * s_noise) * sigma_up : x_euler (sampling.py:144-156,240-247; sampling_utils.py:22-35).
+ * out may alias x. */
+int v3d_ancestral_euler_step(const void* x, const void* den, const void* noise, void* out, float sigma,
+                             float sigma_down, float sigma_up, float sigma_next, float s_noise, int32_t nsamples,
+                             int64_t per_sample, void* stream);
+/* DPM++ 2S ancestral midpoint: out = m1 x - m2 den (sampling.py:257-279).  out may alias x. */
+int v3d_dpmpp2s_stage(const void* x, const void* den, void* out, float m1, float m2, int32_t nsamples,
+                      int64_t per_sample, void* stream);
+/* DPM++ 2S ancestral combine: sigma_down > 0 ? m3 x - m4 den2 : the ancestral Euler step of (x, den), then the
+ * ancestral noise term (sampling.py:265-287).  out may alias x. */
+int v3d_dpmpp2s_step(const void* x, const void* den, const void* den2, const void* noise, void* out, float sigma,
+                     float sigma_down, float sigma_up, float sigma_next, float s_noise, float m3, float m4,
+                     int32_t nsamples, int64_t per_sample, void* stream);
+/* DPM++ 2M: out = m1 x - m2 den, or with second_order != 0: m1 x - m2 (m3 den - m4 hist); then hist := den
+ * (sampling.py:290-345).  out may alias x; hist aliases nothing. */
+int v3d_dpmpp2m_step(const void* x, const void* den, void* hist, void* out, float m1, float m2, float m3, float m4,
+                     int32_t second_order, int32_t nsamples, int64_t per_sample, void* stream);
+/* LMS: ring[slots[0]] := d = (x - den)/sigma; out = x + sum_{j<order} coeffs[j] ring[slots[j]], summed left to right
+ * (sampling.py:194-209).  ring: ring_slots x nsamples x per_sample floats; coeffs / slots are HOST arrays of `order`
+ * entries; 1 <= order <= V3D_LMS_MAX_ORDER <= ring_slots.  out may alias x. */
+int v3d_lms_step(const void* x, const void* den, void* ring, void* out, float sigma, const float* coeffs,
+                 const int32_t* slots, int32_t order, int32_t ring_slots, int32_t nsamples, int64_t per_sample,
+                 void* stream);
 /* clamp((x+1)/2,0,1)*255 -> uint8 THWC from the decoder's NHWC output (scripts/pub/V3D_512.py:286-303). */
 int v3d_decode_to_u8(const void* x, int64_t ldx, int32_t src_fp32, void* y, int64_t npix, void* stream);
 /* same, from NCHW fp32 frames [T][3][HW] (decode_first_stage's return layout) to uint8 [T][HW][3]. */

@@ -1,0 +1,358 @@
+"""EulerAncestralSampler, DPMPP2SAncestralSampler, DPMPP2MSampler and LinearMultistepSampler without a GPU: the oracle
+against the real reference's outputs (tests/golden/edm_small_{euler_ancestral,dpmpp2s,dpmpp2m,lms}.pt, written by
+oracle/make_golden_samplers.py), the drop-in classes' host logic with their step kernels' torch stand-ins
+(tests/sampler_standins.py), and the sharded plans of DiffusionEngine.sample_views over gloo.
+"""
+import json
+import os
+import sys
+from pathlib import Path
+
+import pytest
+import torch
+
+ROOT = str(Path(__file__).resolve().parent.parent)
+sys.path.insert(0, str(Path(__file__).resolve().parent))
+
+GOLD = Path(ROOT) / "tests" / "golden"
+MANIFEST = json.loads((GOLD / "MANIFEST.json").read_text())          # the unet_small weights
+SAMPLERS = json.loads((GOLD / "SAMPLERS.json").read_text())          # the fixtures of oracle/make_golden_samplers.py
+TAGS = ["edm_small_euler_ancestral", "edm_small_dpmpp2s", "edm_small_dpmpp2m", "edm_small_lms"]
+BASE = "v3d_b200.sgm.modules.diffusionmodules."
+UNET_KW = dict(adm_in_channels=768, num_classes="sequential", use_checkpoint=True, in_channels=8, out_channels=4,
+               model_channels=64, attention_resolutions=[4, 2, 1], num_res_blocks=2, channel_mult=[1, 2, 4, 4],
+               num_head_channels=64, use_linear_in_transformer=True, transformer_depth=1, context_dim=1024,
+               spatial_transformer_attn_type="softmax-xformers", extra_ff_mix_layer=True, use_spatial_context=True,
+               merge_strategy="learned_with_images", video_kernel_size=[3, 1, 1])
+
+
+def _rel(a, b):
+    return ((a.float() - b.float()).norm() / b.float().norm().clamp_min(1e-12)).item()
+
+
+def _params(m):
+    """Constructor kwargs of the fixture's sampler beyond the schedule / guider."""
+    return {k: m[k] for k in ("eta", "s_noise", "order") if m.get(k) is not None}
+
+
+def _dropin(shim_cls, m, T, **over):
+    kw = dict(num_steps=m["num_steps"],
+              discretization_config={"target": BASE + "discretizer.EDMDiscretization",
+                                     "params": {"sigma_max": m["sigma_max"]}},
+              guider_config={"target": BASE + "guiders.LinearPredictionGuider",
+                             "params": {"max_scale": m["max_scale"], "min_scale": m["min_scale"], "num_frames": T}})
+    kw.update(_params(m), **over)
+    return shim_cls(**kw)
+
+
+def _counting(fn, box):
+    def wrapped(*a, **k):
+        box[0] += 1
+        return fn(*a, **k)
+    return wrapped
+
+
+@pytest.mark.parametrize("tag", TAGS)
+def test_oracle_restatements_reproduce_reference_golden(tag):
+    from oracle import make_golden_samplers as mgs
+    from oracle import ref_samplers, ref_sampling, ref_unet, synth
+
+    m, mu = SAMPLERS[tag], MANIFEST["unet_small"]
+    gold = torch.load(GOLD / f"{tag}.pt")
+    spec = ref_unet.UNetSpec(model_channels=mu["model_channels"])
+    sd = synth.synth_state_dict(ref_unet.unet_param_shapes(spec), seed=mu["weight_seed"])
+    T, hw, steps = m["T"], m["latent_hw"], m["num_steps"]
+    x, c, uc = synth.synth_inputs(T, hw)
+    extra = {"image_only_indicator": torch.zeros(2, T), "num_video_frames": T}
+
+    def net(i, s, cc):
+        return ref_sampling.denoiser(lambda xx, tt, cond, **k: ref_unet.openai_wrapper(sd, spec, xx, tt, cond, **k),
+                                     i, s, cc, **extra)
+
+    common = (x.clone(), c, uc, steps, ref_sampling.guider_scale(m["min_scale"], m["max_scale"], T), T)
+    with torch.no_grad():
+        if m["sampler"] == "EulerAncestralSampler":
+            out = ref_samplers.euler_ancestral_sample(net, *common, noise_fn=mgs.seeded_noise(m["noise_seed"]),
+                                                      eta=m["eta"], s_noise=m["s_noise"])
+        elif m["sampler"] == "DPMPP2SAncestralSampler":
+            out = ref_samplers.dpmpp2s_ancestral_sample(net, *common, noise_fn=mgs.seeded_noise(m["noise_seed"]),
+                                                        eta=m["eta"], s_noise=m["s_noise"])
+        elif m["sampler"] == "DPMPP2MSampler":
+            out = ref_samplers.dpmpp2m_sample(net, *common)
+        else:
+            out = ref_samplers.lms_sample(net, *common, order=m["order"])
+    assert _rel(out, gold["out"]) <= 1e-6, (tag, _rel(out, gold["out"]))
+
+
+@pytest.mark.parametrize("tag", TAGS)
+def test_dropin_logic_exact_with_fp32_network(tag):
+    """The drop-in samplers (step kernels as stand-ins) around the ORACLE's fp32 UNet reproduce the real reference's
+    outputs to fp32 rounding: schedule, multipliers, skipped evaluations, history and the injected noise, in order.
+    They also evaluate the network exactly as often as the reference did."""
+    import sampler_standins as ss
+    from oracle import make_golden_samplers as mgs
+    from oracle import ref_unet, synth
+    from v3d_b200 import sampling
+
+    m, mu = SAMPLERS[tag], MANIFEST["unet_small"]
+    gold = torch.load(GOLD / f"{tag}.pt")
+    spec = ref_unet.UNetSpec(model_channels=mu["model_channels"])
+    sd = synth.synth_state_dict(ref_unet.unet_param_shapes(spec), seed=mu["weight_seed"])
+    T, hw = m["T"], m["latent_hw"]
+    x, c, uc = synth.synth_inputs(T, hw)
+    sampler = _dropin(ss.CPU_SHIMS[m["sampler"]], m, T)
+    if m.get("noise_seed") is not None:
+        sampler.noise_sampler = mgs.seeded_noise(m["noise_seed"])
+    den = sampling.Denoiser({"target": BASE + "denoiser_scaling.VScalingWithEDMcNoise"})
+
+    class OracleNet(torch.nn.Module):
+        def forward(self, xx, t, cond, **kw):
+            with torch.no_grad():
+                return ref_unet.openai_wrapper(sd, spec, xx, t, cond, **kw)
+
+    extra = {"image_only_indicator": torch.zeros(2, T), "num_video_frames": T}
+    evals = [0]
+    with ss.patched():
+        out = sampler(_counting(lambda i, s, cc: den(OracleNet(), i, s, cc, **extra), evals), x.clone(), cond=c, uc=uc)
+    r = _rel(out, gold["out"])
+    print(tag, "sampler logic with fp32 network vs reference golden: rel-L2", r, "evals", evals[0])
+    assert r <= 1e-5, (tag, r)
+    assert evals[0] == m["network_evals"], (tag, evals[0], m["network_evals"])
+
+
+@pytest.mark.parametrize("tag", TAGS)
+def test_dropin_host_path_with_bf16_unet_matches_reference_golden(tag):
+    """The drop-in samplers through the drop-in Denoiser / OpenAIWrapper / VideoUNet host schedule with every kernel
+    as its CPU stand-in (bf16 network), against the real reference's fp32 outputs: the GPU parity bound, rel-L2 3e-2."""
+    import cpu_shims
+    import sampler_standins as ss
+    from oracle import make_golden_samplers as mgs
+    from oracle import synth
+    from v3d_b200 import sampling
+    from v3d_b200.unet import VideoUNet
+
+    m, mu = SAMPLERS[tag], MANIFEST["unet_small"]
+    gold = torch.load(GOLD / f"{tag}.pt")
+    net = VideoUNet(**dict(UNET_KW, model_channels=mu["model_channels"]))
+    net.load_state_dict(synth.synth_state_dict(net.param_shapes(), seed=mu["weight_seed"]), strict=True)
+    net.__class__ = cpu_shims.CpuUNet
+    T, hw = m["T"], m["latent_hw"]
+    x, c, uc = synth.synth_inputs(T, hw)
+    sampler = _dropin(ss.CPU_SHIMS[m["sampler"]], m, T)
+    if m.get("noise_seed") is not None:
+        sampler.noise_sampler = mgs.seeded_noise(m["noise_seed"])
+    den = sampling.Denoiser({"target": BASE + "denoiser_scaling.VScalingWithEDMcNoise"})
+    model = sampling.OpenAIWrapper(net.eval())
+    extra = {"image_only_indicator": torch.zeros(2, T), "num_video_frames": T}
+    x0 = x.clone()
+    with ss.patched():
+        out = sampler(lambda i, s, cc: den(model, i, s, cc, **extra), x0, cond=c, uc=uc)
+    r = _rel(out, gold["out"])
+    print(tag, "host path vs reference golden: rel-L2", r)
+    assert not torch.equal(x0, x)                       # the caller's noise is scaled in place, like sampling.py:50
+    assert r <= HOST_PATH_BOUND[tag], (tag, r)
+
+
+# Bounds: 2x the measured rel-L2 where it exceeds 1.5e-2.  The sampler logic is exact (the fp32-network test above
+# gives 0.0); what is measured is the bf16 network's rounding carried through the steps down from sigma = 700.
+# Euler-EDM measures 2.2e-2 on the same fixture (test_host_schedule_cpu.py), and the ancestral samplers and LMS land at
+# the same level: Euler-ancestral 2.25e-2, DPM++ 2S 2.24e-2, LMS 2.21e-2.  DPM++ 2M measures 4.8e-2: its
+# second-order step combines two bf16 denoised estimates with weights 1 + 1/(2r) = 2.2 and 1/(2r) = 1.2 (r = h_last / h
+# = 0.42 on this 3-step schedule), which amplifies their rounding.
+HOST_PATH_BOUND = {"edm_small_euler_ancestral": 4.5e-2, "edm_small_dpmpp2s": 4.5e-2, "edm_small_dpmpp2m": 9.6e-2,
+                   "edm_small_lms": 4.4e-2}
+
+
+EVALS_PER_STEPS = {"EulerAncestralSampler": lambda n: n, "DPMPP2SAncestralSampler": lambda n: 2 * n - 1,
+                   "DPMPP2MSampler": lambda n: n, "LinearMultistepSampler": lambda n: n}
+
+
+@pytest.mark.parametrize("name", list(EVALS_PER_STEPS))
+def test_noise_calls_and_network_evaluations(name):
+    """noise_sampler is called once per step with the current state, the last step (sigma_next = 0) included; the
+    network runs N times for N steps (DPM++ 2S: 2N - 1, the last step has no midpoint).  sigma_max 80 keeps every
+    sigma_down of this schedule nonzero in fp32 (a step from 700 straight down to 0.002 rounds it to exactly 0, and the
+    reference then skips that midpoint too)."""
+    import sampler_standins as ss
+
+    T, hw, steps = 3, 4, 4
+    sampler = ss.CPU_SHIMS[name](num_steps=steps, discretization_config={"target": BASE + "discretizer.EDMDiscretization"},
+                                 guider_config={"target": BASE + "guiders.LinearPredictionGuider",
+                                                "params": {"max_scale": 2.5, "num_frames": T}})
+    calls = []
+    if hasattr(sampler, "noise_sampler"):
+        default = sampler.noise_sampler
+        sampler.noise_sampler = lambda x: calls.append(tuple(x.shape)) or default(x)
+    n_eval = [0]
+    g = torch.Generator().manual_seed(0)
+    x = torch.randn(T, 4, hw, hw, generator=g)
+    c = {"crossattn": torch.randn(T, 1, 8, generator=g), "vector": torch.randn(T, 8, generator=g)}
+    with ss.patched():
+        out = sampler(_counting(lambda i, s, cc: 0.5 * i, n_eval), x, cond=c, uc={k: 0 * v for k, v in c.items()})
+    assert torch.isfinite(out).all()
+    assert n_eval[0] == EVALS_PER_STEPS[name](steps), (name, n_eval[0])
+    if name.endswith("AncestralSampler"):
+        assert calls == [(T, 4, hw, hw)] * steps
+    else:
+        assert not hasattr(sampler, "noise_sampler")
+
+
+def test_lms_coefficients_equal_reference_restatement_on_v3d512_schedule():
+    """linear_multistep_coeff (the drop-in's, used once per call) against oracle/ref_samplers.lms_coeff over the
+    float32 V3D_512 schedule (25 steps, sigma_max 700), every order up to 4 and every term."""
+    from oracle import ref_samplers
+    from v3d_b200 import sampling
+    from v3d_b200.sgm.modules.diffusionmodules import sampling_utils
+
+    assert sampling_utils.linear_multistep_coeff is sampling.linear_multistep_coeff
+    t = sampling.EDMDiscretization(sigma_max=700.0)(25).numpy()
+    assert t.dtype.name == "float32"
+    n = 0
+    for i in range(25):
+        for order in range(1, min(i + 1, 4) + 1):
+            for j in range(order):
+                a, b = sampling.linear_multistep_coeff(order, t, i, j), ref_samplers.lms_coeff(order, t, i, j)
+                assert abs(a - b) <= 1e-12 * abs(b), (i, order, j, a, b)
+                n += 1
+    assert n == 1 + 3 + 6 + 22 * 10                 # orders 1..min(i+1, 4), terms j < order
+    with pytest.raises(ValueError):
+        sampling.linear_multistep_coeff(3, t, 1, 0)
+
+
+def test_ancestral_step_helpers_match_reference_formulas():
+    from oracle import ref_samplers
+    from v3d_b200.sgm.modules.diffusionmodules import sampling_utils as su
+
+    s, nxt = torch.tensor([80.0, 3.0]), torch.tensor([3.0, 0.0])
+    down, up = su.get_ancestral_step(s, nxt, eta=0.7)
+    rd, ru = ref_samplers.ancestral_sigmas(s, nxt, 0.7)
+    assert torch.equal(down, rd) and torch.equal(up, ru) and up[1] == 0 and down[1] == 0
+    assert su.get_ancestral_step(s, nxt, eta=0.0) == (nxt, 0.0)
+    x, d = torch.randn(2, 3, 4), torch.randn(2, 3, 4)
+    assert torch.equal(su.to_d(x, s, d), (x - d) / s.reshape(2, 1, 1))
+    assert torch.equal(su.to_sigma(su.to_neg_log_sigma(s)), s.log().neg().neg().exp())
+
+
+@pytest.mark.parametrize("name", ["EulerAncestralSampler", "DPMPP2SAncestralSampler"])
+def test_eta_zero_is_refused(name):
+    """The reference fails at the first ancestral step with eta = 0; the drop-ins refuse it with a clear error."""
+    from v3d_b200 import sampling
+
+    disc = {"target": BASE + "discretizer.EDMDiscretization"}
+    with pytest.raises(ValueError, match="eta = 0"):
+        getattr(sampling, name)(eta=0.0, num_steps=2, discretization_config=disc)
+    smp = getattr(sampling, name)(num_steps=2, discretization_config=disc)
+    smp.eta = 0
+    with pytest.raises(ValueError, match="eta = 0"):
+        smp._loop(lambda i, s, c: i, torch.zeros(1, 4, 2, 2), {})
+
+
+def test_lms_order_above_eight_is_refused():
+    from v3d_b200 import sampling
+
+    disc = {"target": BASE + "discretizer.EDMDiscretization"}
+    sampling.LinearMultistepSampler(order=8, num_steps=2, discretization_config=disc)
+    with pytest.raises(ValueError, match="order 9"):
+        sampling.LinearMultistepSampler(order=9, num_steps=2, discretization_config=disc)
+
+
+def test_cuda_only():
+    from v3d_b200 import sampling
+
+    disc = {"target": BASE + "discretizer.EDMDiscretization"}
+    for name in ("EulerAncestralSampler", "DPMPP2SAncestralSampler", "DPMPP2MSampler", "LinearMultistepSampler"):
+        with pytest.raises(RuntimeError, match="needs CUDA tensors"):
+            getattr(sampling, name)(num_steps=2, discretization_config=disc)(lambda i, s, c: i, torch.zeros(1, 4, 2, 2),
+                                                                              {})
+
+
+def test_targets_resolve():
+    from v3d_b200 import sampling
+
+    for name in ("EulerAncestralSampler", "DPMPP2SAncestralSampler", "DPMPP2MSampler", "LinearMultistepSampler"):
+        assert sampling.get_obj_from_str(BASE + "sampling." + name) is getattr(sampling, name)
+    for name in ("get_ancestral_step", "linear_multistep_coeff", "to_d", "to_neg_log_sigma", "to_sigma"):
+        assert sampling.get_obj_from_str(BASE + "sampling_utils." + name) is getattr(sampling, name)
+    smp = sampling.instantiate_from_config({"target": BASE + "sampling.DPMPP2SAncestralSampler", "params": dict(
+        eta=0.5, s_noise=0.9, num_steps=7, verbose=False, device="cuda",
+        discretization_config={"target": BASE + "discretizer.EDMDiscretization", "params": {"sigma_max": 700.0}},
+        guider_config={"target": BASE + "guiders.LinearPredictionGuider", "params": {"max_scale": 3.5, "num_frames": 18}})})
+    assert (smp.eta, smp.s_noise, smp.num_steps, smp.guider.num_frames) == (0.5, 0.9, 7, 18)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# one image over several ranks (gloo): the injected noise of every rank is its frames of the unsharded draw
+# ---------------------------------------------------------------------------------------------------------------------
+def _expected_evals(name: str, steps: int) -> int:
+    """Network evaluations of the reference for the V3D_512 schedule: DPM++ 2S skips the midpoint wherever the fp32
+    sigma_down is 0."""
+    from v3d_b200 import sampling
+
+    if name != "DPMPP2SAncestralSampler":
+        return steps
+    sig = sampling.EDMDiscretization(sigma_max=700.0)(steps)
+    downs = [sampling.get_ancestral_step(sig[i:i + 1], sig[i + 1:i + 2])[0] for i in range(steps)]
+    return steps + sum(1 for d in downs if float(torch.sum(d)) >= 1e-14)
+
+
+# (sampler, steps) run by every plan; DPM++ 2S over 3 steps evaluates a midpoint on its first step only
+PLAN_SAMPLERS = [("EulerAncestralSampler", 2), ("DPMPP2MSampler", 2), ("DPMPP2SAncestralSampler", 3)]
+
+
+def _plan_worker(rank: int, world: int, port: int, T: int, mode: str, q):
+    sys.path.insert(0, ROOT)
+    sys.path.insert(0, str(Path(ROOT) / "tests"))
+    os.environ.update(RANK=str(rank), LOCAL_RANK=str(rank), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1",
+                      MASTER_PORT=str(port))
+    import torch.distributed as dist
+
+    import sampler_standins as ss
+    from oracle import synth
+    from v3d_b200.viewshard import ShardPlan
+
+    torch.set_num_threads(2)
+    dist.init_process_group("gloo", rank=rank, world_size=world)
+    plan = ShardPlan.create(T, mode)
+    x, c, uc = synth.synth_inputs(T, 8)
+    g = torch.Generator().manual_seed(5)
+    c = dict(c, crossattn=c["crossattn"] + 0.5 * torch.randn(T, 1, 1024, generator=g))
+    res = {"rank": rank, "decode_block": (plan.decode.t0, plan.decode.tl), "cases": {}}
+    for name, steps in PLAN_SAMPLERS:
+        eng, _, _ = ss.cpu_engine(name, T, steps)
+        gathers = plan.cfg.exchanges if plan.cfg is not None else 0
+        with ss.patched():
+            torch.manual_seed(1234)                     # every rank (and the unsharded call) seeds identically
+            ref = eng.sample_views(x.clone(), c, uc, num_frames=T)
+            torch.manual_seed(1234)
+            mine = eng.sample_views(x.clone(), c, uc, num_frames=T, shard=plan)
+            gathered = plan.gather_frames(mine)
+        res["cases"][name] = {"local_rel": _rel(mine, ref[plan.decode.frames]), "gathered_rel": _rel(gathered, ref),
+                              "finite": bool(torch.isfinite(mine).all()),
+                              "cfg_gather": (plan.cfg.exchanges - gathers) if plan.cfg is not None else None,
+                              "engine_sampler_untouched": not hasattr(eng.sampler, "noise_sampler")
+                              or eng.sampler.noise_sampler.__name__ == "<lambda>"}
+    q.put(res)
+    dist.barrier()
+    dist.destroy_process_group()
+
+
+@pytest.mark.parametrize("mode,world,T", [("views", 2, 4), ("cfg", 2, 4), ("cfg+views", 4, 5)])
+def test_sharded_plans_with_noise_injecting_samplers_match_unsharded_gloo(mode, world, T):
+    """EulerAncestralSampler, DPMPP2MSampler and DPMPP2SAncestralSampler through DiffusionEngine.sample_views under
+    ShardPlan 'views', 'cfg' and 'cfg+views' reproduce the unsharded call (rel-L2 <= 1e-6): every rank draws the
+    whole video's noise and keeps its own frames, and the CFG pair gathers once per network evaluation."""
+    from mp_util import run_workers
+
+    res = sorted(run_workers(_plan_worker, world, (T, mode), timeout=1200), key=lambda r: r["rank"])
+    print(res)
+    covered = []
+    for r in res:
+        covered += list(range(r["decode_block"][0], sum(r["decode_block"])))
+        for name, steps in PLAN_SAMPLERS:
+            case = r["cases"][name]
+            assert case["finite"] and case["local_rel"] <= 1e-6 and case["gathered_rel"] <= 1e-6, (name, r)
+            assert case["engine_sampler_untouched"], (name, r)
+            if mode != "views":
+                assert case["cfg_gather"] == _expected_evals(name, steps), (name, case)
+    assert covered == list(range(T))
+    assert _expected_evals("DPMPP2SAncestralSampler", 3) == 4

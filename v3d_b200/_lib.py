@@ -90,6 +90,13 @@ SIGNATURES = {
     "v3d_cfg_combine": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i64, _vp]),
     "v3d_euler_step": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i64, _vp]),
     "v3d_heun_step": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _vp]),
+    "v3d_ancestral_euler_step": (C.c_int, [_vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _f32, _i32, _i64, _vp]),
+    "v3d_dpmpp2s_stage": (C.c_int, [_vp, _vp, _vp, _f32, _f32, _i32, _i64, _vp]),
+    "v3d_dpmpp2s_step": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _f32, _f32, _f32, _i32, _i64,
+                                   _vp]),
+    "v3d_dpmpp2m_step": (C.c_int, [_vp, _vp, _vp, _vp, _f32, _f32, _f32, _f32, _i32, _i32, _i64, _vp]),
+    "v3d_lms_step": (C.c_int, [_vp, _vp, _vp, _vp, _f32, C.POINTER(C.c_float), C.POINTER(C.c_int32), _i32, _i32,
+                               _i32, _i64, _vp]),
     "v3d_decode_to_u8": (C.c_int, [_vp, _i64, _i32, _vp, _i64, _vp]),
     "v3d_frames_nchw_to_u8": (C.c_int, [_vp, _vp, _i32, _i64, _vp]),
 }

@@ -90,6 +90,92 @@ __global__ void heun_step_kernel(const float* __restrict__ x, const float* __res
   }
 }
 
+// The ancestral / DPM++ / LMS steps below round every operation separately (__f*_rn: no FMA contraction), in the
+// order of the reference's torch expressions, so that they reproduce its fp32 results bit for bit.
+
+// x + (noise * s_noise) * sigma_up where sigma_next > 0, else x   (AncestralSampler.ancestral_step)
+__device__ __forceinline__ float add_ancestral_noise(float x, const float* __restrict__ noise, long long i,
+                                                     float s_noise, float sigma_up, float sigma_next) {
+  return sigma_next > 0.0f ? __fadd_rn(x, __fmul_rn(__fmul_rn(noise[i], s_noise), sigma_up)) : x;
+}
+
+// d = (x - den) / sigma; x_euler = x + (sigma_down - sigma) * d; then the ancestral noise term
+__global__ void ancestral_euler_step_kernel(const float* __restrict__ x, const float* __restrict__ den,
+                                            const float* __restrict__ noise, float* __restrict__ out, float sigma,
+                                            float sigma_down, float sigma_up, float sigma_next, float s_noise,
+                                            long long total) {
+  const float dt = __fsub_rn(sigma_down, sigma);
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const float xi = x[i];
+    const float d = __fdiv_rn(__fsub_rn(xi, den[i]), sigma);
+    out[i] = add_ancestral_noise(__fadd_rn(xi, __fmul_rn(dt, d)), noise, i, s_noise, sigma_up, sigma_next);
+  }
+}
+
+// out = m1 * x - m2 * den   (DPM++ 2S midpoint, DPM++ 2M first-order step)
+__global__ void dpm_first_order_kernel(const float* __restrict__ x, const float* __restrict__ den,
+                                       float* __restrict__ out, float m1, float m2, long long total) {
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x)
+    out[i] = __fsub_rn(__fmul_rn(m1, x[i]), __fmul_rn(m2, den[i]));
+}
+
+// sigma_down > 0 ? m3 * x - m4 * den2 : x_euler(x, den); then the ancestral noise term
+__global__ void dpmpp2s_step_kernel(const float* __restrict__ x, const float* __restrict__ den,
+                                    const float* __restrict__ den2, const float* __restrict__ noise,
+                                    float* __restrict__ out, float sigma, float sigma_down, float sigma_up,
+                                    float sigma_next, float s_noise, float m3, float m4, long long total) {
+  const float dt = __fsub_rn(sigma_down, sigma);
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const float xi = x[i];
+    float r;
+    if (sigma_down > 0.0f) {
+      r = __fsub_rn(__fmul_rn(m3, xi), __fmul_rn(m4, den2[i]));
+    } else {
+      const float d = __fdiv_rn(__fsub_rn(xi, den[i]), sigma);
+      r = __fadd_rn(xi, __fmul_rn(dt, d));
+    }
+    out[i] = add_ancestral_noise(r, noise, i, s_noise, sigma_up, sigma_next);
+  }
+}
+
+// x_std = m1 x - m2 D; with history and sigma_next > 0: m1 x - m2 (m3 D - m4 D_old).  hist <- D afterwards.
+__global__ void dpmpp2m_step_kernel(const float* __restrict__ x, const float* __restrict__ den, float* hist,
+                                    float* out, float m1, float m2, float m3, float m4, int second_order,
+                                    long long total) {
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const float xi = x[i], di = den[i];
+    float dd = di;
+    if (second_order) dd = __fsub_rn(__fmul_rn(m3, di), __fmul_rn(m4, hist[i]));
+    hist[i] = di;
+    out[i] = __fsub_rn(__fmul_rn(m1, xi), __fmul_rn(m2, dd));
+  }
+}
+
+struct LmsTerms {
+  float c[V3D_LMS_MAX_ORDER];
+  int slot[V3D_LMS_MAX_ORDER];
+};
+
+// ring[slot[0]] <- d = (x - den) / sigma;  out = x + (((c0 d_i + c1 d_{i-1}) + c2 d_{i-2}) + ...)
+__global__ void lms_step_kernel(const float* x, const float* __restrict__ den, float* ring, float* out, float sigma,
+                                LmsTerms terms, int order, long long total) {
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const float xi = x[i];
+    const float d = __fdiv_rn(__fsub_rn(xi, den[i]), sigma);
+    ring[terms.slot[0] * total + i] = d;
+    float acc = __fmul_rn(terms.c[0], d);
+#pragma unroll
+    for (int j = 1; j < V3D_LMS_MAX_ORDER; ++j)
+      if (j < order) acc = __fadd_rn(acc, __fmul_rn(terms.c[j], ring[terms.slot[j] * total + i]));
+    out[i] = __fadd_rn(xi, acc);
+  }
+}
+
 // frames[p][c] = uint8(clamp((x[p][c] + 1) / 2, 0, 1) * 255)  (truncating cast, like numpy astype)
 template <typename T>
 __global__ void decode_to_u8_kernel(const T* __restrict__ x, long long ldx, uint8_t* __restrict__ y, long long npix) {
@@ -195,6 +281,104 @@ int v3d_heun_step(const void* x, const void* den, const void* x_euler, const voi
       static_cast<const float*>(den2), static_cast<const float*>(sigma_hat), static_cast<const float*>(sigma_next),
       static_cast<float*>(out), nsamples, per_sample);
   V3D_CHECK_LAUNCH("heun_step_kernel");
+  return V3D_OK;
+}
+
+/* EulerAncestralSampler.sampler_step: AncestralSampler.ancestral_euler_step + ancestral_step (sampling.py:144-156,
+ * 240-247) with sigma_down / sigma_up of get_ancestral_step (sampling_utils.py:22-31).  out may alias x. */
+int v3d_ancestral_euler_step(const void* x, const void* den, const void* noise, void* out, float sigma,
+                             float sigma_down, float sigma_up, float sigma_next, float s_noise, int32_t nsamples,
+                             int64_t per_sample, void* stream) {
+  if (!x || !den || !noise || !out || nsamples <= 0 || per_sample <= 0 || !(sigma > 0.0f)) {
+    set_error("v3d_ancestral_euler_step: bad args");
+    return V3D_ERR_BAD_ARG;
+  }
+  const long long total = nsamples * per_sample;
+  ancestral_euler_step_kernel<<<ew_blocks(total), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const float*>(x), static_cast<const float*>(den), static_cast<const float*>(noise),
+      static_cast<float*>(out), sigma, sigma_down, sigma_up, sigma_next, s_noise, total);
+  V3D_CHECK_LAUNCH("ancestral_euler_step_kernel");
+  return V3D_OK;
+}
+
+/* DPMPP2SAncestralSampler.sampler_step midpoint (sampling.py:257-279): x2 = m1 * x - m2 * den with
+ * m1 = sigma(s) / sigma(t), m2 = expm1(-h / 2).  out may alias x. */
+int v3d_dpmpp2s_stage(const void* x, const void* den, void* out, float m1, float m2, int32_t nsamples,
+                      int64_t per_sample, void* stream) {
+  if (!x || !den || !out || nsamples <= 0 || per_sample <= 0) {
+    set_error("v3d_dpmpp2s_stage: bad args");
+    return V3D_ERR_BAD_ARG;
+  }
+  const long long total = nsamples * per_sample;
+  dpm_first_order_kernel<<<ew_blocks(total), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const float*>(x), static_cast<const float*>(den), static_cast<float*>(out), m1, m2, total);
+  V3D_CHECK_LAUNCH("dpm_first_order_kernel");
+  return V3D_OK;
+}
+
+/* DPMPP2SAncestralSampler.sampler_step final combine (sampling.py:265-287): sigma_down > 0 ? m3 * x - m4 * den2 :
+ * the ancestral Euler step of (x, den), then ancestral_step's noise term; m3 = sigma(t_next) / sigma(t),
+ * m4 = expm1(-h), den2 = denoised(x2, sigma(s)).  out may alias x. */
+int v3d_dpmpp2s_step(const void* x, const void* den, const void* den2, const void* noise, void* out, float sigma,
+                     float sigma_down, float sigma_up, float sigma_next, float s_noise, float m3, float m4,
+                     int32_t nsamples, int64_t per_sample, void* stream) {
+  if (!x || !den || !den2 || !noise || !out || nsamples <= 0 || per_sample <= 0 || !(sigma > 0.0f)) {
+    set_error("v3d_dpmpp2s_step: bad args");
+    return V3D_ERR_BAD_ARG;
+  }
+  const long long total = nsamples * per_sample;
+  dpmpp2s_step_kernel<<<ew_blocks(total), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const float*>(x), static_cast<const float*>(den), static_cast<const float*>(den2),
+      static_cast<const float*>(noise), static_cast<float*>(out), sigma, sigma_down, sigma_up, sigma_next, s_noise,
+      m3, m4, total);
+  V3D_CHECK_LAUNCH("dpmpp2s_step_kernel");
+  return V3D_OK;
+}
+
+/* DPMPP2MSampler.sampler_step (sampling.py:290-345): m1 = sigma(t_next) / sigma(t), m2 = expm1(-h);
+ * second_order != 0 (previous step exists and sigma_next > 0): m3 = 1 + 1/(2r), m4 = 1/(2r) with the previous
+ * denoised estimate read from hist.  hist is overwritten with den (the next step's old_denoised).  out may alias x;
+ * hist must not alias x, den or out. */
+int v3d_dpmpp2m_step(const void* x, const void* den, void* hist, void* out, float m1, float m2, float m3, float m4,
+                     int32_t second_order, int32_t nsamples, int64_t per_sample, void* stream) {
+  if (!x || !den || !hist || !out || nsamples <= 0 || per_sample <= 0) {
+    set_error("v3d_dpmpp2m_step: bad args");
+    return V3D_ERR_BAD_ARG;
+  }
+  const long long total = nsamples * per_sample;
+  dpmpp2m_step_kernel<<<ew_blocks(total), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const float*>(x), static_cast<const float*>(den), static_cast<float*>(hist),
+      static_cast<float*>(out), m1, m2, m3, m4, second_order, total);
+  V3D_CHECK_LAUNCH("dpmpp2m_step_kernel");
+  return V3D_OK;
+}
+
+/* LinearMultistepSampler.__call__ loop body (sampling.py:194-209): ring holds `ring_slots` slopes of
+ * nsamples * per_sample floats each; d = (x - den) / sigma is stored in slot slots[0], then
+ * out = x + sum_j coeffs[j] * ring[slots[j]] for j < order (slots[j] = the slot of d_{i-j}; coeffs, slots: host
+ * arrays of `order` entries, order <= V3D_LMS_MAX_ORDER).  out may alias x. */
+int v3d_lms_step(const void* x, const void* den, void* ring, void* out, float sigma, const float* coeffs,
+                 const int32_t* slots, int32_t order, int32_t ring_slots, int32_t nsamples, int64_t per_sample,
+                 void* stream) {
+  if (!x || !den || !ring || !out || !coeffs || !slots || nsamples <= 0 || per_sample <= 0 || !(sigma > 0.0f) ||
+      order < 1 || order > V3D_LMS_MAX_ORDER || ring_slots < order) {
+    set_error("v3d_lms_step: bad args (order must be 1..8 and fit the ring)");
+    return V3D_ERR_BAD_ARG;
+  }
+  LmsTerms terms{};
+  for (int j = 0; j < order; ++j) {
+    if (slots[j] < 0 || slots[j] >= ring_slots) {
+      set_error("v3d_lms_step: ring slot out of range");
+      return V3D_ERR_BAD_ARG;
+    }
+    terms.c[j] = coeffs[j];
+    terms.slot[j] = slots[j];
+  }
+  const long long total = nsamples * per_sample;
+  lms_step_kernel<<<ew_blocks(total), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const float*>(x), static_cast<const float*>(den), static_cast<float*>(ring),
+      static_cast<float*>(out), sigma, terms, order, total);
+  V3D_CHECK_LAUNCH("lms_step_kernel");
   return V3D_OK;
 }
 

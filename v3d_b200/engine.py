@@ -153,7 +153,13 @@ class DiffusionEngine(nn.Module):
         ONE image over several ranks: `shard` = a v3d_b200.viewshard.ShardPlan (frame blocks, CFG-pair split, or both;
         `view_shard=ViewShard` is shorthand for the frame-block plan).  Every rank passes the SAME full-video randn / c /
         uc and gets back the decoded frames of its own block [t_local,3,8h,8w]; `gather_frames` of the plan (or of the
-        ViewShard) assembles the video.  The video is decoded as one chunk (decoding_t = T)."""
+        ViewShard) assembles the video.  The video is decoded as one chunk (decoding_t = T).
+
+        Samplers that inject noise every step (those with a `noise_sampler`: EulerAncestralSampler,
+        DPMPP2SAncestralSampler) draw it, on every rank, for the WHOLE video - `noise_sampler` is called on a [T, ...]
+        tensor - and keep this rank's frames of the draw.  So all ranks must start from the same generator state (seed
+        them identically, as they already pass the identical `randn`); they then inject exactly the noise of the
+        unsharded call."""
         if view_shard is not None and shard is None:
             from .viewshard import ShardPlan
 
@@ -198,6 +204,14 @@ class DiffusionEngine(nn.Module):
         sampler = copy.copy(self.sampler)
         guider = vs.shard_guider(self.sampler.guider) if vs is not None else self.sampler.guider
         sampler.guider = CfgSplitGuider(guider, cs) if cs is not None else guider
+        if getattr(sampler, "noise_sampler", None) is not None:
+            draw_full = sampler.noise_sampler
+
+            def noise_sampler(x_local):
+                # the unsharded draw, restricted to this rank's frames (see sample_views)
+                return draw_full(x_local.new_empty((num_frames,) + tuple(x_local.shape[1:])))[frames]
+
+            sampler.noise_sampler = noise_sampler
         try:
             unet.view_shard = vs
             z = sampler(denoiser, x, cond=c_l, uc=uc_l)       # this rank's sampling frames, identical across a CFG pair

@@ -358,6 +358,57 @@ def heun_step(x, den, x_euler, den2, sigma_hat, sigma_next, out, nsamples: int, 
     return out
 
 
+def _need_f32(who: str, **tensors) -> None:
+    for name, t in tensors.items():
+        _need(t, torch.float32, f"{who} {name}")
+
+
+def ancestral_euler_step(x, den, noise, out, sigma: float, sigma_down: float, sigma_up: float, sigma_next: float,
+                         s_noise: float, nsamples: int, per_sample: int):
+    _need_f32("ancestral_euler_step", x=x, den=den, noise=noise, out=out)
+    _lib.check(_lib.load().v3d_ancestral_euler_step(x.data_ptr(), den.data_ptr(), noise.data_ptr(), out.data_ptr(),
+                                                    sigma, sigma_down, sigma_up, sigma_next, s_noise, nsamples,
+                                                    per_sample, _stream()), "v3d_ancestral_euler_step")
+    return out
+
+
+def dpmpp2s_stage(x, den, out, m1: float, m2: float, nsamples: int, per_sample: int):
+    _need_f32("dpmpp2s_stage", x=x, den=den, out=out)
+    _lib.check(_lib.load().v3d_dpmpp2s_stage(x.data_ptr(), den.data_ptr(), out.data_ptr(), m1, m2, nsamples,
+                                             per_sample, _stream()), "v3d_dpmpp2s_stage")
+    return out
+
+
+def dpmpp2s_step(x, den, den2, noise, out, sigma: float, sigma_down: float, sigma_up: float, sigma_next: float,
+                 s_noise: float, m3: float, m4: float, nsamples: int, per_sample: int):
+    _need_f32("dpmpp2s_step", x=x, den=den, den2=den2, noise=noise, out=out)
+    _lib.check(_lib.load().v3d_dpmpp2s_step(x.data_ptr(), den.data_ptr(), den2.data_ptr(), noise.data_ptr(),
+                                            out.data_ptr(), sigma, sigma_down, sigma_up, sigma_next, s_noise, m3, m4,
+                                            nsamples, per_sample, _stream()), "v3d_dpmpp2s_step")
+    return out
+
+
+def dpmpp2m_step(x, den, hist, out, m1: float, m2: float, m3: float, m4: float, second_order: bool, nsamples: int,
+                 per_sample: int):
+    _need_f32("dpmpp2m_step", x=x, den=den, hist=hist, out=out)
+    _lib.check(_lib.load().v3d_dpmpp2m_step(x.data_ptr(), den.data_ptr(), hist.data_ptr(), out.data_ptr(), m1, m2,
+                                            m3, m4, 1 if second_order else 0, nsamples, per_sample, _stream()),
+               "v3d_dpmpp2m_step")
+    return out
+
+
+def lms_step(x, den, ring, out, sigma: float, coeffs, slots, nsamples: int, per_sample: int):
+    """ring: [ring_slots, *x.shape]; coeffs[j] multiplies the slope stored in ring[slots[j]] (slots[0] receives this
+    step's slope)."""
+    _need_f32("lms_step", x=x, den=den, ring=ring, out=out)
+    order = len(coeffs)
+    c_arr = (C.c_float * max(order, 1))(*coeffs)
+    s_arr = (C.c_int32 * max(order, 1))(*slots)
+    _lib.check(_lib.load().v3d_lms_step(x.data_ptr(), den.data_ptr(), ring.data_ptr(), out.data_ptr(), sigma, c_arr,
+                                        s_arr, order, ring.shape[0], nsamples, per_sample, _stream()), "v3d_lms_step")
+    return out
+
+
 def decode_to_u8(x: torch.Tensor, ldx: int, y: torch.Tensor, npix: int):
     _lib.check(_lib.load().v3d_decode_to_u8(x.data_ptr(), ldx, 1 if x.dtype == torch.float32 else 0,
                                             y.data_ptr(), npix, _stream()), "v3d_decode_to_u8")

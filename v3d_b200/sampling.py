@@ -3,7 +3,8 @@
 `VScalingWithEDMcNoise` + `Denoiser` (denoiser_scaling.py:51-59, denoiser.py:12-39), `OpenAIWrapper`
 (wrappers.py:9-34), `EulerEDMSampler` (sampling.py:24-133,214-218) and - SURVEY 8(f)-3, same denoiser, no new
 tensor-core work - `HeunEDMSampler` (sampling.py:221-237), `VanillaCFG` (guiders.py:23-42) and
-`CentralPredictionGuider` (guiders.py:104-146).
+`CentralPredictionGuider` (guiders.py:104-146); `EulerAncestralSampler`, `DPMPP2SAncestralSampler`, `DPMPP2MSampler`,
+`LinearMultistepSampler` (sampling.py:136-211,240-365) with the helpers of sampling_utils.py:7-43.
 
 Call shapes are the reference's: `sampler(denoiser, x, cond=c, uc=uc) -> x`, `denoiser(network, input, sigma,
 cond, **kw)`, `network(x, t, c, **kw)`; any denoiser closure works (scripts/pub/V3D_512.py:278-283).  The
@@ -338,5 +339,264 @@ class HeunEDMSampler(EulerEDMSampler):
                 x = self.sampler_step(sig_rows[i], sig_rows[i + 1], denoiser, x, cond, uc, gamma)
         finally:
             self._next_sigma_host = None
+        return x
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# sampling_utils.py:7-43 (also exported at v3d_b200.sgm.modules.diffusionmodules.sampling_utils)
+# ---------------------------------------------------------------------------------------------------------------------
+def _append_dims(v: torch.Tensor, ndim: int) -> torch.Tensor:
+    if v.ndim > ndim:
+        raise ValueError(f"input has {v.ndim} dims but target_dims is {ndim}, which is less")
+    return v.reshape(tuple(v.shape) + (1,) * (ndim - v.ndim))
+
+
+def linear_multistep_coeff(order: int, t, i: int, j: int, epsrel: float = 1e-4) -> float:
+    """Integral over [t[i], t[i+1]] of the Lagrange basis polynomial of node t[i-j] on the nodes t[i], ..., t[i-order+1]
+    (sampling_utils.py:7-19).  `t` is the float32 numpy schedule, as the reference passes it: the integrand then runs in
+    float32 and the adaptive quadrature sees exactly the reference's values."""
+    from scipy import integrate
+
+    if order - 1 > i:
+        raise ValueError(f"Order {order} too high for step {i}")
+    nodes = [k for k in range(order) if k != j]
+
+    def basis(tau):
+        prod = 1.0
+        for k in nodes:
+            prod *= (tau - t[i - k]) / (t[i - j] - t[i - k])
+        return prod
+
+    return integrate.quad(basis, t[i], t[i + 1], epsrel=epsrel)[0]
+
+
+def get_ancestral_step(sigma_from: torch.Tensor, sigma_to: torch.Tensor, eta: float = 1.0):
+    """(sigma_down, sigma_up) of an ancestral step with noise fraction eta (sampling_utils.py:22-31)."""
+    if not eta:
+        return sigma_to, 0.0
+    sigma_up = torch.minimum(sigma_to, eta * (sigma_to ** 2 * (sigma_from ** 2 - sigma_to ** 2) / sigma_from ** 2) ** 0.5)
+    sigma_down = (sigma_to ** 2 - sigma_up ** 2) ** 0.5
+    return sigma_down, sigma_up
+
+
+def to_d(x: torch.Tensor, sigma: torch.Tensor, denoised: torch.Tensor) -> torch.Tensor:
+    return (x - denoised) / _append_dims(sigma, x.ndim)
+
+
+def to_neg_log_sigma(sigma: torch.Tensor) -> torch.Tensor:
+    return sigma.log().neg()
+
+
+def to_sigma(neg_log_sigma: torch.Tensor) -> torch.Tensor:
+    return neg_log_sigma.neg().exp()
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Ancestral, DPM++ and linear-multistep samplers (sampling.py:136-211,240-365)
+# ---------------------------------------------------------------------------------------------------------------------
+LMS_MAX_ORDER = 8  # V3D_LMS_MAX_ORDER of include/v3d_b200.h
+
+
+def _f32(v: float) -> torch.Tensor:
+    """One schedule value as the fp32 tensor the reference computes its multipliers with (every sample of a step shares
+    the step's sigma, so one element stands for the reference's `s_in * sigmas[i]`)."""
+    return torch.tensor([v], dtype=torch.float32)
+
+
+def _sigma_rows(values: List[float], n: int, device) -> torch.Tensor:
+    """[len(values), n] fp32 per-sample sigma rows for the denoiser, uploaded once per call from pinned memory without a
+    host sync."""
+    rows = torch.tensor(values, dtype=torch.float32).reshape(-1, 1).expand(len(values), n).contiguous()
+    if torch.device(device).type == "cuda":
+        return rows.pin_memory().to(device, non_blocking=True)
+    return rows
+
+
+class _ScheduleSampler:
+    """BaseDiffusionSampler (sampling.py:24-74) for the samplers below: the sigma schedule and every multiplier derived
+    from it live on the host (computed in fp32 with the reference's expressions), the state, the denoised estimates and
+    the sampler history on the device; each step's arithmetic is one native kernel (csrc/sampler.cu)."""
+
+    def __init__(self, discretization_config, num_steps: Optional[int] = None, guider_config=None,
+                 verbose: bool = False, device: str = "cuda"):
+        self.num_steps = num_steps
+        self.discretization = instantiate_from_config(discretization_config)
+        self.guider = instantiate_from_config(guider_config if guider_config is not None else DEFAULT_GUIDER)
+        self.verbose = verbose
+        self.device = device
+
+    prepare_sampling_loop = EulerEDMSampler.prepare_sampling_loop
+
+    def denoise(self, x, denoiser, sigma, cond, uc, **kwargs):
+        denoised = denoiser(*self.guider.prepare_inputs(x, sigma, cond, uc), **kwargs)
+        return self.guider(denoised, sigma).float().contiguous()
+
+    def _steps(self, num_sigmas: int):
+        steps = range(num_sigmas - 1)
+        if self.verbose:
+            from tqdm import tqdm
+
+            steps = tqdm(steps, total=num_sigmas - 1, desc=f"Sampling with {type(self).__name__}")
+        return steps
+
+    def __call__(self, denoiser, x, cond, uc=None, num_steps=None, **kwargs):
+        if not x.is_cuda:
+            raise RuntimeError(f"v3d_b200.{type(self).__name__} needs CUDA tensors; there is no CPU fallback")
+        return self._loop(denoiser, x, cond, uc, num_steps, **kwargs)
+
+    def _start(self, x, cond, uc, num_steps):
+        assert x.dtype == torch.float32, "sampler state is fp32 (denoiser.py:36-39)"
+        x, sigmas, num_sigmas, cond, uc = self.prepare_sampling_loop(x, cond, uc, num_steps)
+        return x.contiguous(), sigmas.float(), num_sigmas, cond, uc
+
+
+class _AncestralSampler(_ScheduleSampler):
+    """AncestralSampler (sampling.py:136-173).  `noise_sampler(x)` is called once per step with the current state,
+    the last step included (where ancestral_step discards the draw because sigma_next = 0), so a caller who replaces it
+    or seeds torch's generator gets the reference's draws in the reference's order.
+
+    eta = 0 is refused: the reference fails at the first step there (get_ancestral_step returns the python float 0.0
+    as sigma_up and append_dims cannot take it, sampling_utils.py:24, util.py:194-201)."""
+
+    def __init__(self, eta: float = 1.0, s_noise: float = 1.0, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.eta = eta
+        self.s_noise = s_noise
+        self.noise_sampler = lambda x: torch.randn_like(x)
+        self._check_eta()
+
+    def _check_eta(self) -> None:
+        if not self.eta:
+            raise ValueError(f"{type(self).__name__}: eta = 0 is not supported (the reference sampler fails on it); "
+                             "use eta > 0, or DPMPP2MSampler / EulerEDMSampler for deterministic sampling")
+
+    def _ancestral(self, sigma: float, sigma_next: float):
+        sigma_down, sigma_up = get_ancestral_step(_f32(sigma), _f32(sigma_next), eta=self.eta)
+        return sigma_down, sigma_up
+
+    def _noise(self, x: torch.Tensor) -> torch.Tensor:
+        noise = self.noise_sampler(x)
+        if tuple(noise.shape) != tuple(x.shape) or noise.device != x.device:
+            raise RuntimeError(f"noise_sampler returned {tuple(noise.shape)} on {noise.device}; expected "
+                               f"{tuple(x.shape)} on {x.device}")
+        return noise.float().contiguous()
+
+
+class EulerAncestralSampler(_AncestralSampler):
+    """sampling.py:240-247: one network evaluation per step; v3d_ancestral_euler_step does the Euler step to
+    sigma_down and adds the sigma_up noise."""
+
+    def _loop(self, denoiser, x, cond, uc=None, num_steps=None):
+        self._check_eta()
+        x, sigmas, num_sigmas, cond, uc = self._start(x, cond, uc, num_steps)
+        n, per = x.shape[0], x[0].numel()
+        host = [float(s) for s in sigmas]
+        rows = _sigma_rows(host, n, x.device)
+        out = torch.empty_like(x)          # the caller's (scaled) noise is not overwritten, like the reference
+        for i in self._steps(num_sigmas):
+            sigma_down, sigma_up = self._ancestral(host[i], host[i + 1])
+            den = self.denoise(x, denoiser, rows[i], cond, uc)
+            ops.ancestral_euler_step(x, den, self._noise(x), out, host[i], float(sigma_down), float(sigma_up),
+                                     host[i + 1], self.s_noise, n, per)
+            x = out
+        return x
+
+
+class DPMPP2SAncestralSampler(_AncestralSampler):
+    """sampling.py:250-287: a midpoint evaluation at sigma(s) = sqrt(sigma * sigma_down) and the second-order update,
+    except where every sigma_down is 0 (the last step), which takes the ancestral Euler step instead and saves the
+    evaluation: 2N - 1 network evaluations for N steps."""
+
+    def _loop(self, denoiser, x, cond, uc=None, num_steps=None):
+        self._check_eta()
+        x, sigmas, num_sigmas, cond, uc = self._start(x, cond, uc, num_steps)
+        n, per = x.shape[0], x[0].numel()
+        host = [float(s) for s in sigmas]
+        plan, mid_sigmas = [], []
+        for i in range(num_sigmas - 1):
+            sigma_down, sigma_up = self._ancestral(host[i], host[i + 1])
+            step = {"down": float(sigma_down), "up": float(sigma_up), "mid": None}
+            if float(sigma_down) * n >= 1e-14:          # torch.sum(sigma_down) < 1e-14 skips the midpoint
+                t, t_next = to_neg_log_sigma(_f32(host[i])), to_neg_log_sigma(sigma_down)
+                h = t_next - t
+                s = t + 0.5 * h
+                step.update(mid=len(mid_sigmas), m1=float(to_sigma(s) / to_sigma(t)), m2=float((-0.5 * h).expm1()),
+                            m3=float(to_sigma(t_next) / to_sigma(t)), m4=float((-h).expm1()))
+                mid_sigmas.append(float(to_sigma(s)))
+            plan.append(step)
+        rows = _sigma_rows(host[:-1] + mid_sigmas, n, x.device)
+        out, x2 = torch.empty_like(x), torch.empty_like(x)
+        for i in self._steps(num_sigmas):
+            p = plan[i]
+            den = self.denoise(x, denoiser, rows[i], cond, uc)
+            if p["mid"] is None:
+                ops.ancestral_euler_step(x, den, self._noise(x), out, host[i], p["down"], p["up"], host[i + 1],
+                                         self.s_noise, n, per)
+            else:
+                ops.dpmpp2s_stage(x, den, x2, p["m1"], p["m2"], n, per)
+                den2 = self.denoise(x2, denoiser, rows[num_sigmas - 1 + p["mid"]], cond, uc)
+                ops.dpmpp2s_step(x, den, den2, self._noise(x), out, host[i], p["down"], p["up"], host[i + 1],
+                                 self.s_noise, p["m3"], p["m4"], n, per)
+            x = out
+        return x
+
+
+class DPMPP2MSampler(_ScheduleSampler):
+    """sampling.py:290-365: one network evaluation per step; the previous denoised estimate stays on the device
+    (v3d_dpmpp2m_step reads it and stores the new one).  The first step and a step to sigma_next = 0 are first order."""
+
+    def _loop(self, denoiser, x, cond, uc=None, num_steps=None, **kwargs):
+        # extra keyword arguments are accepted and ignored, as by the reference's __call__ (sampling.py:347)
+        x, sigmas, num_sigmas, cond, uc = self._start(x, cond, uc, num_steps)
+        n, per = x.shape[0], x[0].numel()
+        host = [float(s) for s in sigmas]
+        rows = _sigma_rows(host, n, x.device)
+        out, old_denoised = torch.empty_like(x), torch.empty_like(x)
+        for i in self._steps(num_sigmas):
+            t, t_next = to_neg_log_sigma(_f32(host[i])), to_neg_log_sigma(_f32(host[i + 1]))
+            h = t_next - t
+            m1, m2 = float(to_sigma(t_next) / to_sigma(t)), float((-h).expm1())
+            m3 = m4 = 0.0
+            second_order = i > 0 and host[i + 1] * n >= 1e-14
+            if second_order:
+                r = (t - to_neg_log_sigma(_f32(host[i - 1]))) / h
+                m3, m4 = float(1 + 1 / (2 * r)), float(1 / (2 * r))
+            den = self.denoise(x, denoiser, rows[i], cond, uc)
+            ops.dpmpp2m_step(x, den, old_denoised, out, m1, m2, m3, m4, second_order, n, per)
+            x = out
+        return x
+
+
+class LinearMultistepSampler(_ScheduleSampler):
+    """sampling.py:176-211: one network evaluation per step; the last `order` slopes d = (x - D) / sigma live in a
+    device ring and the linear_multistep_coeff weights are integrated on the host once per call.  order is at most
+    LMS_MAX_ORDER (8)."""
+
+    def __init__(self, order: int = 4, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        if not 1 <= int(order) <= LMS_MAX_ORDER:
+            raise ValueError(f"LinearMultistepSampler: order {order} is outside 1..{LMS_MAX_ORDER}")
+        self.order = int(order)
+
+    def _loop(self, denoiser, x, cond, uc=None, num_steps=None, **kwargs):
+        if not 1 <= int(self.order) <= LMS_MAX_ORDER:
+            raise ValueError(f"LinearMultistepSampler: order {self.order} is outside 1..{LMS_MAX_ORDER}")
+        order = int(self.order)
+        x, sigmas, num_sigmas, cond, uc = self._start(x, cond, uc, num_steps)
+        n, per = x.shape[0], x[0].numel()
+        host = [float(s) for s in sigmas]
+        sigmas_np = sigmas.numpy()
+        coeffs = []
+        for i in range(num_sigmas - 1):
+            cur = min(i + 1, order)
+            coeffs.append([linear_multistep_coeff(cur, sigmas_np, i, j) for j in range(cur)])
+        rows = _sigma_rows(host, n, x.device)
+        out = torch.empty_like(x)
+        ring = torch.empty((order,) + tuple(x.shape), device=x.device, dtype=torch.float32)
+        for i in self._steps(num_sigmas):
+            den = self.denoise(x, denoiser, rows[i], cond, uc, **kwargs)
+            slots = [(i - j) % order for j in range(len(coeffs[i]))]
+            ops.lms_step(x, den, ring, out, host[i], coeffs[i], slots, n, per)
+            x = out
         return x
 

@@ -273,22 +273,27 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     }
     const int obase = n_tile * OUT_COLS;  // first output column of this tile
     const int nbase = n_tile * BN;        // first column in the (packed) N space
+    // operand pointers at this thread's first column (cq), so that every load of the unrolled column loop below is
+    // one instruction with an immediate offset instead of a re-derived address
+    const float* bcol = has_bias && EPI != EPI_TRANS ? p.bias + nbase + cq : nullptr;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int tr = tr_base + 8 * h;
       long long row = 0;
       const bool valid = map_row(tr, t0, t1, t2, row);
-      const float* fb = nullptr;
-      const bf16* r1p = nullptr;
-      const bf16* r2p = nullptr;
+      // Rows past the end (tail tiles) read row 0 of the per-frame bias and the residuals instead: their results are
+      // never stored (the TMA store clips them, the fp32 stores check `valid`), and the column loop then branches on
+      // launch-uniform flags only.
+      const long long orow = valid ? row : 0;
+      const float* fb = has_fb ? p.fbias + static_cast<long long>(static_cast<int>(orow) / p.rows_per_frame) * p.ldfb +
+                                     nbase + cq
+                               : nullptr;
+      const bf16* r1p = has_r1 ? p.R1 + orow * p.ldr1 + obase + cq : nullptr;
+      const bf16* r2p = has_r2 ? p.R2 + orow * p.ldr2 + obase + cq : nullptr;
       float row_bias = 0.f;
-      if (valid) {
-        if (has_fb) fb = p.fbias + static_cast<long long>(static_cast<int>(row) / p.rows_per_frame) * p.ldfb + nbase;
-        if (has_r1) r1p = p.R1 + row * p.ldr1 + obase;
-        if (has_r2) r2p = p.R2 + row * p.ldr2 + obase;
-        if (EPI == EPI_TRANS && has_bias) row_bias = __ldg(p.bias + row);
-      }
+      if (EPI == EPI_TRANS && has_bias && valid) row_bias = __ldg(p.bias + row);
       const uint32_t swz = SUBW == 32 ? static_cast<uint32_t>((tr >> 1) & 3) : 0u;  // 64B-swizzle XOR of the chunk
+      const uint32_t srow = stg + static_cast<uint32_t>(tr * SUBW * 2 + cq * 2);  // staged row, this thread's column
 #pragma unroll
       for (int j = 0; j < OUT_COLS / 8; ++j) {
         const int oc = 8 * j + cq;
@@ -297,19 +302,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
           v0 += row_bias;
           v1 += row_bias;
         } else if (has_bias) {
-          v0 += __ldg(p.bias + nbase + oc);
-          v1 += __ldg(p.bias + nbase + oc + 1);
+          v0 += __ldg(bcol + 8 * j);
+          v1 += __ldg(bcol + 8 * j + 1);
         }
-        if (fb) {
-          v0 += __ldg(fb + oc);
-          v1 += __ldg(fb + oc + 1);
+        if (has_fb) {
+          v0 += __ldg(fb + 8 * j);
+          v1 += __ldg(fb + 8 * j + 1);
         }
         if (GEGLU) {
           constexpr int JG = BN / 16;  // the gate of column c is column c + BN / 2 of the packed tile
           float g0 = acc[4 * (j + JG) + 2 * h], g1 = acc[4 * (j + JG) + 2 * h + 1];
           if (has_bias) {
-            g0 += __ldg(p.bias + nbase + BN / 2 + oc);
-            g1 += __ldg(p.bias + nbase + BN / 2 + oc + 1);
+            g0 += __ldg(bcol + BN / 2 + 8 * j);
+            g1 += __ldg(bcol + BN / 2 + 8 * j + 1);
           }
           v0 *= gelu_erf_fast(g0);
           v1 *= gelu_erf_fast(g1);
@@ -317,21 +322,21 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
           v0 = silu_f(v0);
           v1 = silu_f(v1);
         }
-        if (r1p || r2p) {
-          if (r1p) {
-            const float2 x = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(r1p + oc)));
+        if (has_r1 || has_r2) {
+          if (has_r1) {
+            const float2 x = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(r1p + 8 * j)));
             v0 = fmaf(v0, s0, x.x * s1);
             v1 = fmaf(v1, s0, x.y * s1);
           } else {
             v0 *= s0;
             v1 *= s0;
           }
-          if (r2p) {
-            const float2 x = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(r2p + oc)));
+          if (has_r2) {
+            const float2 x = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(r2p + 8 * j)));
             v0 = fmaf(x.x, s2, v0);
             v1 = fmaf(x.y, s2, v1);
           }
-        } else if (s0 != 1.0f) {
+        } else {  // s0 = 1 scales exactly
           v0 *= s0;
           v1 *= s0;
         }
@@ -351,10 +356,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
           if (valid)
             *reinterpret_cast<float2*>(static_cast<float*>(p.D) + row * p.ldd + obase + oc) = make_float2(v0, v1);
         } else {
-          const int sub = oc / SUBW;
-          const int cc = oc - sub * SUBW;
-          const uint32_t addr = stg + static_cast<uint32_t>(sub * C::SUB_BYTES + tr * SUBW * 2) +
-                                ((static_cast<uint32_t>(cc >> 3) ^ swz) << 4) + static_cast<uint32_t>((cc & 7) * 2);
+          // sub-tile and 16-byte chunk of column 8 j + cq fold to constants once j is unrolled (cq < 8, SUBW % 8 == 0)
+          const int sub = 8 * j / SUBW;
+          const int chunk = (8 * j - sub * SUBW) >> 3;
+          const uint32_t addr = srow + static_cast<uint32_t>(sub * C::SUB_BYTES) + ((static_cast<uint32_t>(chunk) ^ swz) << 4);
           asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_bf16x2(v0, v1)) : "memory");
         }
       }

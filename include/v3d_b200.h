@@ -137,6 +137,30 @@ int64_t v3d_groupnorm_workspace_bytes(void);
 int v3d_groupnorm(const void* x, void* y, const void* gamma, const void* beta, int64_t rows_per_sample,
                   int32_t nsamples, int32_t C, int32_t ldx, int32_t groups, float eps, int32_t silu,
                   void* workspace, int64_t workspace_bytes, void* stream);
+/* Deterministic GroupNorm (opt-in): statistics that depend on the shape and the data only, never on the launch grid,
+ * nsamples or a sharded plan.  A sample's rows_per_sample = frames x hw rows are cut into blocks of min(256, hw) rows
+ * that never straddle a frame (the last block of a frame may be short); each (block, group) gets one fp32
+ * (sum, sumsq) pair from a fixed in-CTA tree; the pairs are folded in fp64 in block order (lane l of one warp adds
+ * blocks l, l + 32, ..., then an xor-shuffle tree).  The same shape and data give the same bits on the same GPU model
+ * and library build.  hw = H*W for 2-D norms and for the 3-D time_stack norms alike.
+ *   v3d_groupnorm_det_blocks            blocks per sample (-1 if hw does not divide rows_per_sample); host function
+ *   v3d_groupnorm_partials              the block partials: float2 [nsamples][ldp][groups], ldp >= blocks per sample
+ *   v3d_groupnorm_fold_apply            fold the nblocks partials of each sample ([nsamples][nblocks][groups]) over
+ *                                       count_rows x C/groups elements, then y (dense, ld = C) = act(GN(x)); a frame-
+ *                                       sharded caller passes the whole video's partials and count_rows
+ *   v3d_groupnorm_det                   both in one launch (grid barrier), bit-identical to the pair; workspace >=
+ *                                       v3d_groupnorm_det_workspace_bytes(...) bytes, zeroed once by the caller and
+ *                                       passed unchanged to every call on the same stream */
+int64_t v3d_groupnorm_det_blocks(int64_t rows_per_sample, int64_t hw);
+int64_t v3d_groupnorm_det_workspace_bytes(int64_t rows_per_sample, int64_t hw, int32_t nsamples, int32_t groups);
+int v3d_groupnorm_partials(const void* x, void* partials, int64_t rows_per_sample, int64_t hw, int32_t nsamples,
+                           int32_t C, int32_t ldx, int32_t groups, int64_t ldp, void* stream);
+int v3d_groupnorm_fold_apply(const void* x, void* y, const void* partials, const void* gamma, const void* beta,
+                             int64_t rows_per_sample, int32_t nsamples, int32_t C, int32_t ldx, int32_t groups,
+                             int64_t nblocks, int64_t count_rows, float eps, int32_t silu, void* stream);
+int v3d_groupnorm_det(const void* x, void* y, const void* gamma, const void* beta, int64_t rows_per_sample, int64_t hw,
+                      int32_t nsamples, int32_t C, int32_t ldx, int32_t groups, float eps, int32_t silu,
+                      void* workspace, int64_t workspace_bytes, void* stream);
 /* LayerNorm over C (attention.py:525-527; video_attention.py:51,79,93-94). Optional fused
  * z = x + add[row / rows_per_frame] (fp32 vectors; video_attention.py:286-287), z stored to ysum. */
 int v3d_layernorm(const void* x, const void* add, void* ysum, void* y, const void* gamma, const void* beta,

@@ -54,6 +54,13 @@ SIGNATURES = {
     "v3d_groupnorm_apply": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _f32, _i32, _vp]),
     "v3d_groupnorm_workspace_bytes": (C.c_int64, []),
     "v3d_groupnorm": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _f32, _i32, _vp, _i64, _vp]),
+    "v3d_groupnorm_det_blocks": (C.c_int64, [_i64, _i64]),
+    "v3d_groupnorm_det_workspace_bytes": (C.c_int64, [_i64, _i64, _i32, _i32]),
+    "v3d_groupnorm_partials": (C.c_int, [_vp, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _i64, _vp]),
+    "v3d_groupnorm_fold_apply": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _i64, _i64, _f32,
+                                           _i32, _vp]),
+    "v3d_groupnorm_det": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _f32, _i32, _vp, _i64,
+                                    _vp]),
     "v3d_layernorm": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _f32, _vp]),
     "v3d_softmax_rows": (C.c_int, [_vp, _i64, _i32, _f32, _vp]),
     "v3d_softmax_rows_f32": (C.c_int, [_vp, _vp, _i64, _i32, _f32, _vp]),

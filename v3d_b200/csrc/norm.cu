@@ -337,6 +337,254 @@ gn_fused_kernel(const bf16* __restrict__ x, bf16* __restrict__ y, const float* _
 }
 
 // ------------------------------------------------------------------------------------------------
+// Deterministic GroupNorm (opt-in).  ONE definition of the statistics, whatever the launch geometry:
+//   blocks   a sample's rows, [frames][hw], are cut into blocks of R = min(256, hw) rows; a block never straddles a
+//            frame and the last block of a frame may be short (nbf = ceil(hw / R) blocks per frame);
+//   partial  each (block, group) gets ONE fp32 (sum, sumsq) pair from a fixed in-CTA tree: every thread sums its
+//            8-channel column over the block's rows in row order, then one warp per group adds the group's
+//            (channel, row lane) sums lane-strided and folds the lanes with an xor-shuffle tree;
+//   fold     per (sample, group), in fp64: lane l of one warp adds blocks l, l + 32, l + 64, ... in turn, then an
+//            xor-shuffle tree folds the 32 lanes.
+// The statistics depend on the shape and the data only - not on the grid, on nsamples, on a CFG split or on which rank
+// computed which frames (the partials of a frame subset equal those of the same frames inside the whole tensor), so
+// the two-kernel form, the single-launch form and every sharded plan produce the same bits.
+// ------------------------------------------------------------------------------------------------
+constexpr long long kGnDetRows = 256;
+
+__host__ __device__ __forceinline__ long long gn_det_block_rows(long long hw) { return hw < kGnDetRows ? hw : kGnDetRows; }
+__host__ __device__ __forceinline__ long long gn_det_blocks_per_frame(long long hw) {
+  const long long r = gn_det_block_rows(hw);
+  return (hw + r - 1) / r;
+}
+// rows [r0, r1) of block `blk` of a sample
+__device__ __forceinline__ void gn_det_block_range(long long blk, long long hw, long long& r0, long long& r1) {
+  const long long nbf = gn_det_blocks_per_frame(hw), R = gn_det_block_rows(hw);
+  const long long f = blk / nbf, b = blk - f * nbf;
+  r0 = f * hw + b * R;
+  r1 = r0 + R < (f + 1) * hw ? r0 + R : (f + 1) * hw;
+}
+
+// (sum, sumsq) of rows [r0, r1) of one sample (xs = its first row) for every group -> part[g].  Called by every
+// thread of the CTA (it synchronises); s_red = [2][lanes_r][C] floats.
+__device__ __forceinline__ void gn_det_block_partial(const bf16* __restrict__ xs, long long r0, long long r1,
+                                                     long long ldx, int C, int groups, float* s_red,
+                                                     float2* __restrict__ part) {
+  const int vpr = C >> 3;
+  const int lanes_r = blockDim.x / vpr;
+  const int vc = threadIdx.x % vpr;
+  const int rl = threadIdx.x / vpr;
+  const int cg = C / groups;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+  const bf16* xb = xs + vc * 8;
+  float s[8], q[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) s[j] = q[j] = 0.f;
+  auto accum = [&](const uint4& u) {
+    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 f = unpack_bf16x2(w[j]);
+      s[2 * j] += f.x; q[2 * j] = fmaf(f.x, f.x, q[2 * j]);
+      s[2 * j + 1] += f.y; q[2 * j + 1] = fmaf(f.y, f.y, q[2 * j + 1]);
+    }
+  };
+  long long r = r0 + rl;
+  for (; r + static_cast<long long>(kGnUnroll - 1) * lanes_r < r1; r += static_cast<long long>(kGnUnroll) * lanes_r) {
+    uint4 u[kGnUnroll];
+#pragma unroll
+    for (int k = 0; k < kGnUnroll; ++k)
+      u[k] = __ldg(reinterpret_cast<const uint4*>(xb + (r + static_cast<long long>(k) * lanes_r) * ldx));
+#pragma unroll
+    for (int k = 0; k < kGnUnroll; ++k) accum(u[k]);
+  }
+  for (; r < r1; r += lanes_r) accum(__ldg(reinterpret_cast<const uint4*>(xb + r * ldx)));
+  __syncthreads();  // the previous block's tree may still be reading s_red
+  {
+    float* ss = s_red + (static_cast<size_t>(rl) * C + vc * 8);
+    float* qq = ss + static_cast<size_t>(lanes_r) * C;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      ss[j] = s[j];
+      qq[j] = q[j];
+    }
+  }
+  __syncthreads();
+  for (int g = warp < nwarps ? warp : groups; g < groups; g += nwarps) {
+    float a = 0.f, b = 0.f;
+    const int n = cg * lanes_r;
+    for (int i = lane; i < n; i += 32) {
+      const int rr = i / cg, cc = g * cg + (i - rr * cg);
+      a += s_red[static_cast<size_t>(rr) * C + cc];
+      b += s_red[static_cast<size_t>(lanes_r + rr) * C + cc];
+    }
+    a = warp_sum(a);
+    b = warp_sum(b);
+    if (lane == 0) part[g] = make_float2(a, b);
+  }
+}
+
+// mean / rstd of every group of one sample from its nblk block partials ([nblk][groups]) -> s_stat[groups][2].
+// One warp per group; the fold order depends on nblk only.  The caller synchronises before reading s_stat.
+__device__ __forceinline__ void gn_det_fold(const float2* __restrict__ part, long long nblk, int groups, double cnt,
+                                            float eps, float* s_stat) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+  for (int g = warp < nwarps ? warp : groups; g < groups; g += nwarps) {
+    double a = 0.0, b = 0.0;
+    for (long long k = lane; k < nblk; k += 32) {
+      const float2 p = __ldcg(&part[k * groups + g]);
+      a += static_cast<double>(p.x);
+      b += static_cast<double>(p.y);
+    }
+    a = warp_sum_f64(a);
+    b = warp_sum_f64(b);
+    if (lane == 0) {
+      const double mean = a / cnt;
+      double var = b / cnt - mean * mean;
+      if (var < 0.0) var = 0.0;
+      s_stat[2 * g] = static_cast<float>(mean);
+      s_stat[2 * g + 1] = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
+    }
+  }
+}
+
+// y rows [r0, r1) = act(x * sc + sh) for this thread's 8-channel column (xb / yb: the sample's first row + column)
+__device__ __forceinline__ void gn_det_apply_rows(const bf16* __restrict__ xb, bf16* __restrict__ yb, long long r0,
+                                                  long long r1, long long ldx, int C, const float* sc, const float* sh,
+                                                  int silu) {
+  const int vpr = C >> 3;
+  const int lanes_r = blockDim.x / vpr;
+  const int rl = threadIdx.x / vpr;
+  auto emit = [&](const uint4& u, long long rr) {
+    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+    uint32_t o[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 f = unpack_bf16x2(w[j]);
+      float a = fmaf(f.x, sc[2 * j], sh[2 * j]);
+      float b = fmaf(f.y, sc[2 * j + 1], sh[2 * j + 1]);
+      if (silu) {
+        a = silu_f(a);
+        b = silu_f(b);
+      }
+      o[j] = pack_bf16x2(a, b);
+    }
+    *reinterpret_cast<uint4*>(yb + rr * static_cast<long long>(C)) = make_uint4(o[0], o[1], o[2], o[3]);
+  };
+  long long r = r0 + rl;
+  for (; r + static_cast<long long>(kGnUnroll - 1) * lanes_r < r1; r += static_cast<long long>(kGnUnroll) * lanes_r) {
+    uint4 u[kGnUnroll];
+#pragma unroll
+    for (int k = 0; k < kGnUnroll; ++k)
+      u[k] = __ldg(reinterpret_cast<const uint4*>(xb + (r + static_cast<long long>(k) * lanes_r) * ldx));
+#pragma unroll
+    for (int k = 0; k < kGnUnroll; ++k) emit(u[k], r + static_cast<long long>(k) * lanes_r);
+  }
+  for (; r < r1; r += lanes_r) emit(__ldg(reinterpret_cast<const uint4*>(xb + r * ldx)), r);
+}
+
+// per-thread scale / shift of its 8 channels from s_stat
+__device__ __forceinline__ void gn_det_scale_shift(const float* s_stat, const float* __restrict__ gamma,
+                                                   const float* __restrict__ beta, int C, int groups, float* sc,
+                                                   float* sh) {
+  const int vc = threadIdx.x % (C >> 3);
+  const int cg = C / groups;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int c = vc * 8 + j;
+    const int g = c / cg;
+    const float a = s_stat[2 * g + 1] * __ldg(gamma + c);
+    sc[j] = a;
+    sh[j] = __ldg(beta + c) - s_stat[2 * g] * a;
+  }
+}
+
+// grid = (blocks per sample, samples): one CTA per block
+__global__ void __launch_bounds__(512)
+gn_det_partials_kernel(const bf16* __restrict__ x, float2* __restrict__ partial, long long rows_per_sample,
+                       long long hw, int C, long long ldx, int groups, long long ldp) {
+  extern __shared__ float s_red[];  // [2][lanes_r][C]
+  const int sample = blockIdx.y;
+  long long r0, r1;
+  gn_det_block_range(blockIdx.x, hw, r0, r1);
+  gn_det_block_partial(x + static_cast<long long>(sample) * rows_per_sample * ldx, r0, r1, ldx, C, groups, s_red,
+                       partial + (static_cast<long long>(sample) * ldp + blockIdx.x) * groups);
+}
+
+// grid = (row chunks, samples): every CTA folds its sample's partials, then normalises its rows
+__global__ void __launch_bounds__(512)
+gn_det_apply_kernel(const bf16* __restrict__ x, bf16* __restrict__ y, const float2* __restrict__ partial,
+                    const float* __restrict__ gamma, const float* __restrict__ beta, long long rows_per_sample, int C,
+                    long long ldx, int groups, long long nblk, long long count_rows, float eps, int silu,
+                    int rows_per_cta) {
+  __shared__ float s_stat[64];  // [groups <= 32][2]
+  const int sample = blockIdx.y;
+  gn_det_fold(partial + static_cast<long long>(sample) * nblk * groups, nblk, groups,
+              static_cast<double>(count_rows) * (C / groups), eps, s_stat);
+  __syncthreads();
+  float sc[8], sh[8];
+  gn_det_scale_shift(s_stat, gamma, beta, C, groups, sc, sh);
+  const long long row0 = static_cast<long long>(blockIdx.x) * rows_per_cta;
+  long long row1 = row0 + rows_per_cta;
+  if (row1 > rows_per_sample) row1 = rows_per_sample;
+  const long long srow = static_cast<long long>(sample) * rows_per_sample;
+  const int vc = threadIdx.x % (C >> 3);
+  gn_det_apply_rows(x + srow * ldx + vc * 8, y + srow * static_cast<long long>(C) + vc * 8, row0, row1, ldx, C, sc, sh,
+                    silu);
+}
+
+// Single launch, deterministic: the CTAs of a sample stride over its blocks (CTA i takes blocks i, i + gridDim.x, ...)
+// and write the block partials, a grid-wide barrier, then EVERY CTA folds all blocks of its sample (so the fold does
+// not depend on gridDim) and normalises the rows of its own blocks, last block first (the rows read last are the ones
+// most likely still in L2).
+template <int MAXT, int MINB>
+__global__ void __launch_bounds__(MAXT, MINB)
+gn_det_fused_kernel(const bf16* __restrict__ x, bf16* __restrict__ y, const float* __restrict__ gamma,
+                    const float* __restrict__ beta, GnBarrier* __restrict__ bar, float2* __restrict__ partial,
+                    long long rows_per_sample, long long hw, int C, long long ldx, int groups, float eps, int silu) {
+  extern __shared__ float s_red[];  // [2][lanes_r][C] thread partials, reused as [groups][2] mean / rstd
+  const int sample = blockIdx.y;
+  const long long nblk = rows_per_sample / hw * gn_det_blocks_per_frame(hw);
+  const bf16* xs = x + static_cast<long long>(sample) * rows_per_sample * ldx;
+  float2* ps = partial + static_cast<long long>(sample) * nblk * groups;
+  for (long long blk = blockIdx.x; blk < nblk; blk += gridDim.x) {
+    long long r0, r1;
+    gn_det_block_range(blk, hw, r0, r1);
+    gn_det_block_partial(xs, r0, r1, ldx, C, groups, s_red, ps + blk * groups);
+  }
+  // grid-wide barrier (sense reversal, as in gn_fused_kernel)
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const unsigned int total = gridDim.x * gridDim.y;
+    const unsigned int my_gen = ld_acquire_u32(&bar->gen);
+    __threadfence();
+    const unsigned int prev = atomicAdd(&bar->count, 1u);
+    if (prev == total - 1) {
+      bar->count = 0;
+      __threadfence();
+      st_release_u32(&bar->gen, my_gen + 1);
+    } else {
+      while (ld_acquire_u32(&bar->gen) == my_gen) __nanosleep(64);
+    }
+  }
+  __syncthreads();
+  float* s_stat = s_red;
+  gn_det_fold(ps, nblk, groups, static_cast<double>(rows_per_sample) * (C / groups), eps, s_stat);
+  __syncthreads();
+  float sc[8], sh[8];
+  gn_det_scale_shift(s_stat, gamma, beta, C, groups, sc, sh);
+  const int vc = threadIdx.x % (C >> 3);
+  const bf16* xb = xs + vc * 8;
+  bf16* yb = y + static_cast<long long>(sample) * rows_per_sample * C + vc * 8;
+  if (static_cast<long long>(blockIdx.x) >= nblk) return;
+  const long long last = blockIdx.x + (nblk - 1 - blockIdx.x) / gridDim.x * gridDim.x;
+  for (long long blk = last; blk >= 0; blk -= gridDim.x) {
+    long long r0, r1;
+    gn_det_block_range(blk, hw, r0, r1);
+    gn_det_apply_rows(xb, yb, r0, r1, ldx, C, sc, sh, silu);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // LayerNorm over C (<= 2048), one warp per row, row held in registers.
 //   z = x[row] + add[row / rows_per_frame]   (add optional, fp32)
 //   ysum[row] = bf16(z)                      (optional)
@@ -757,6 +1005,114 @@ int v3d_groupnorm(const void* x, void* y, const void* gamma, const void* beta, i
       static_cast<const float*>(beta), reinterpret_cast<GnBarrier*>(ws), reinterpret_cast<float2*>(ws + 256),
       rows_per_sample, C, ldx, groups, eps, silu, static_cast<int>(rpc));
   V3D_CHECK_LAUNCH("gn_fused_kernel");
+  return V3D_OK;
+}
+
+/* Deterministic GroupNorm: blocks per sample of the statistics definition (rows_per_sample = frames x hw, blocks of
+ * min(256, hw) rows that never straddle a frame); -1 if hw does not divide rows_per_sample. */
+int64_t v3d_groupnorm_det_blocks(int64_t rows_per_sample, int64_t hw) {
+  if (hw <= 0 || rows_per_sample <= 0 || rows_per_sample % hw != 0) return -1;
+  return rows_per_sample / hw * gn_det_blocks_per_frame(hw);
+}
+
+/* Bytes of the workspace v3d_groupnorm_det needs for this shape (barrier words + one fp32 pair per block and group). */
+int64_t v3d_groupnorm_det_workspace_bytes(int64_t rows_per_sample, int64_t hw, int32_t nsamples, int32_t groups) {
+  const int64_t nblk = v3d_groupnorm_det_blocks(rows_per_sample, hw);
+  if (nblk < 0 || nsamples <= 0 || groups <= 0) return -1;
+  return 256 + static_cast<int64_t>(sizeof(float2)) * nblk * nsamples * groups;
+}
+
+static bool gn_det_args_ok(const void* x, int64_t rows_per_sample, int64_t hw, int32_t nsamples, int32_t C, int32_t ldx,
+                           int32_t groups) {
+  return x && C % 8 == 0 && groups > 0 && groups <= 32 && C % groups == 0 && C / 8 <= 512 && ldx % 8 == 0 &&
+         nsamples > 0 && v3d_groupnorm_det_blocks(rows_per_sample, hw) > 0;
+}
+
+/* Block partials of the deterministic statistics: partials = float2 [nsamples][ldp][groups], block k of sample s at
+ * [s][k] (k < v3d_groupnorm_det_blocks(rows_per_sample, hw) <= ldp). */
+int v3d_groupnorm_partials(const void* x, void* partials, int64_t rows_per_sample, int64_t hw, int32_t nsamples,
+                           int32_t C, int32_t ldx, int32_t groups, int64_t ldp, void* stream) {
+  const int64_t nblk = v3d_groupnorm_det_blocks(rows_per_sample, hw);
+  if (!gn_det_args_ok(x, rows_per_sample, hw, nsamples, C, ldx, groups) || !partials || ldp < nblk ||
+      nsamples > 65535) {
+    set_error("v3d_groupnorm_partials: bad args C=%d groups=%d ldx=%d hw=%lld ldp=%lld", C, groups, ldx,
+              static_cast<long long>(hw), static_cast<long long>(ldp));
+    return V3D_ERR_BAD_ARG;
+  }
+  const int vpr = C / 8;
+  const int lanes_r = kGnThreads / vpr > 0 ? kGnThreads / vpr : 1;
+  gn_det_partials_kernel<<<dim3(static_cast<unsigned>(nblk), nsamples), vpr * lanes_r,
+                           sizeof(float) * 2 * static_cast<size_t>(lanes_r) * C, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const bf16*>(x), static_cast<float2*>(partials), rows_per_sample, hw, C, ldx, groups, ldp);
+  V3D_CHECK_LAUNCH("gn_det_partials_kernel");
+  return V3D_OK;
+}
+
+/* y[dense, ld=C] = act(GroupNorm(x)) from block partials: each sample's nblocks pairs (float2 [nsamples][nblocks]
+ * [groups]) are folded in block order, over count_rows x C/groups elements (count_rows = rows the partials cover: the
+ * whole video's when x holds one rank's frames of it). */
+int v3d_groupnorm_fold_apply(const void* x, void* y, const void* partials, const void* gamma, const void* beta,
+                             int64_t rows_per_sample, int32_t nsamples, int32_t C, int32_t ldx, int32_t groups,
+                             int64_t nblocks, int64_t count_rows, float eps, int32_t silu, void* stream) {
+  if (!gn_det_args_ok(x, rows_per_sample, rows_per_sample, nsamples, C, ldx, groups) || !y || !partials || !gamma ||
+      !beta || nblocks <= 0 || count_rows <= 0 || nsamples > 65535) {
+    set_error("v3d_groupnorm_fold_apply: bad args C=%d groups=%d ldx=%d nblocks=%lld", C, groups, ldx,
+              static_cast<long long>(nblocks));
+    return V3D_ERR_BAD_ARG;
+  }
+  const int rpc = pick_rows_per_cta(rows_per_sample, nsamples);
+  const int vpr = C / 8;
+  const int lanes_r = kGnThreads / vpr > 0 ? kGnThreads / vpr : 1;
+  gn_det_apply_kernel<<<dim3(static_cast<unsigned>((rows_per_sample + rpc - 1) / rpc), nsamples), vpr * lanes_r, 0,
+                        static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const bf16*>(x), static_cast<bf16*>(y), static_cast<const float2*>(partials),
+      static_cast<const float*>(gamma), static_cast<const float*>(beta), rows_per_sample, C, ldx, groups, nblocks,
+      count_rows, eps, silu, rpc);
+  V3D_CHECK_LAUNCH("gn_det_apply_kernel");
+  return V3D_OK;
+}
+
+/* The deterministic normalisation in ONE launch; bit-identical to v3d_groupnorm_partials + v3d_groupnorm_fold_apply.
+ * workspace: >= v3d_groupnorm_det_workspace_bytes(rows_per_sample, hw, nsamples, groups) bytes, zeroed once by the
+ * caller, then passed unchanged to every call on the same stream. */
+int v3d_groupnorm_det(const void* x, void* y, const void* gamma, const void* beta, int64_t rows_per_sample, int64_t hw,
+                      int32_t nsamples, int32_t C, int32_t ldx, int32_t groups, float eps, int32_t silu,
+                      void* workspace, int64_t workspace_bytes, void* stream) {
+  const int64_t need = v3d_groupnorm_det_workspace_bytes(rows_per_sample, hw, nsamples, groups);
+  if (!gn_det_args_ok(x, rows_per_sample, hw, nsamples, C, ldx, groups) || !y || !gamma || !beta || !workspace ||
+      workspace_bytes < need) {
+    set_error("v3d_groupnorm_det: bad args C=%d groups=%d ldx=%d hw=%lld workspace=%lld (need %lld)", C, groups, ldx,
+              static_cast<long long>(hw), static_cast<long long>(workspace_bytes), static_cast<long long>(need));
+    return V3D_ERR_BAD_ARG;
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int vpr = C / 8;
+  const int lanes_r = kGnThreads / vpr > 0 ? kGnThreads / vpr : 1;
+  const int threads = vpr * lanes_r;
+  size_t smem = sizeof(float) * 2 * static_cast<size_t>(lanes_r) * C;
+  if (smem < sizeof(float) * 2 * groups) smem = sizeof(float) * 2 * groups;
+  int per_sm = 0;
+  auto kern = threads <= 256 ? gn_det_fused_kernel<256, 3> : gn_det_fused_kernel<512, 1>;
+  cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem);
+  if (e != cudaSuccess || per_sm < 1) {
+    set_error("v3d_groupnorm_det: occupancy query failed (%s)", cudaGetErrorString(e));
+    return V3D_ERR_CUDA;
+  }
+  if (per_sm > 4) per_sm = 4;
+  const long long cap = static_cast<long long>(per_sm) * num_sms();
+  if (nsamples > cap) {
+    set_error("v3d_groupnorm_det: %d samples exceed the co-resident grid (%lld CTAs)", nsamples, cap);
+    return V3D_ERR_UNSUPPORTED;
+  }
+  long long chunks = cap / nsamples;
+  const long long nblk = v3d_groupnorm_det_blocks(rows_per_sample, hw);
+  if (chunks > nblk) chunks = nblk;
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  kern<<<dim3(static_cast<unsigned>(chunks), nsamples), threads, smem, st>>>(
+      static_cast<const bf16*>(x), static_cast<bf16*>(y), static_cast<const float*>(gamma),
+      static_cast<const float*>(beta), reinterpret_cast<GnBarrier*>(ws), reinterpret_cast<float2*>(ws + 256),
+      rows_per_sample, hw, C, ldx, groups, eps, silu);
+  V3D_CHECK_LAUNCH("gn_det_fused_kernel");
   return V3D_OK;
 }
 

@@ -233,11 +233,11 @@ class VideoDecoder(KernelModule):
         ts = name + ".time_stack"
         norm = self._gn_halo if self.view_shard is not None else None
         a = (norm(P, ts + ".in_layers.0", xs, hw, T, nb, co, 1e-5, True) if norm else
-             self._gn(P, ts + ".in_layers.0", xs, T * hw, nb, co, 1e-5, True))
+             self._gn(P, ts + ".in_layers.0", xs, T * hw, nb, co, 1e-5, True, hw=hw))
         h2 = torch.empty(rows, co, device=x.device, dtype=torch.bfloat16)
         self._tconv(P, ts + ".in_layers.2", a, h2, hw, T, nb, co)
         a = (norm(P, ts + ".out_layers.0", h2, hw, T, nb, co, 1e-5, True) if norm else
-             self._gn(P, ts + ".out_layers.0", h2, T * hw, nb, co, 1e-5, True))
+             self._gn(P, ts + ".out_layers.0", h2, T * hw, nb, co, 1e-5, True, hw=hw))
         self._tconv(P, ts + ".out_layers.3", a, h2, hw, T, nb, co, r1=xs, s1=1.0, s0=P[name + ".alpha"])
         return h2
 

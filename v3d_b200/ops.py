@@ -7,6 +7,7 @@ Activations are bf16 token-major / NHWC ([rows, C]); see DESIGN.md for the layou
 from __future__ import annotations
 
 import ctypes as C
+import os
 from typing import Optional
 
 import torch
@@ -148,6 +149,74 @@ def groupnorm(x: torch.Tensor, y: torch.Tensor, gamma: torch.Tensor, beta: torch
                                          rows_per_sample, nsamples, c, c if ldx is None else ldx, groups, eps,
                                          1 if silu else 0, workspace.data_ptr(), workspace.numel(), _stream()),
                "v3d_groupnorm")
+    return y
+
+
+def deterministic() -> bool:
+    """Deterministic mode: on under torch.use_deterministic_algorithms(True) or V3D_DETERMINISTIC=1.  The modules then
+    take the GroupNorm statistics from the block partials below, which do not depend on the launch grid, nsamples or a
+    sharded plan; every other kernel is deterministic in both modes."""
+    return torch.are_deterministic_algorithms_enabled() or os.environ.get("V3D_DETERMINISTIC", "0") == "1"
+
+
+def groupnorm_det_blocks(rows_per_sample: int, hw: int) -> int:
+    """Blocks per sample of the deterministic statistics (rows of min(256, hw), never straddling a frame)."""
+    n = int(_lib.load().v3d_groupnorm_det_blocks(rows_per_sample, hw))
+    if n <= 0:
+        raise RuntimeError(f"groupnorm_det_blocks: hw={hw} does not divide rows_per_sample={rows_per_sample}")
+    return n
+
+
+def groupnorm_det_workspace_bytes(rows_per_sample: int, hw: int, nsamples: int, groups: int = 32) -> int:
+    return int(_lib.load().v3d_groupnorm_det_workspace_bytes(rows_per_sample, hw, nsamples, groups))
+
+
+def groupnorm_partials(x: torch.Tensor, partials: torch.Tensor, rows_per_sample: int, hw: int, nsamples: int, c: int,
+                       ldx: Optional[int] = None, groups: int = 32, ldp: Optional[int] = None) -> torch.Tensor:
+    """partials: fp32 [nsamples, ldp, groups, 2] (a view may start at a block offset of a wider buffer; ldp = its
+    blocks per sample, default: this shape's)."""
+    _need(x, torch.bfloat16, "groupnorm x")
+    _need(partials, torch.float32, "groupnorm partials")
+    ldp = groupnorm_det_blocks(rows_per_sample, hw) if ldp is None else ldp
+    _lib.check(_lib.load().v3d_groupnorm_partials(x.data_ptr(), partials.data_ptr(), rows_per_sample, hw, nsamples, c,
+                                                  c if ldx is None else ldx, groups, ldp, _stream()),
+               "v3d_groupnorm_partials")
+    return partials
+
+
+def groupnorm_fold_apply(x: torch.Tensor, y: torch.Tensor, partials: torch.Tensor, gamma: torch.Tensor,
+                         beta: torch.Tensor, rows_per_sample: int, nsamples: int, c: int, eps: float, silu: bool,
+                         nblocks: int, count_rows: Optional[int] = None, ldx: Optional[int] = None,
+                         groups: int = 32) -> torch.Tensor:
+    """y = act(GroupNorm(x)) with the statistics folded from `nblocks` block partials per sample; count_rows = the rows
+    they cover (default rows_per_sample; the whole video's when x holds one rank's frames)."""
+    _need(x, torch.bfloat16, "groupnorm x")
+    _need(partials, torch.float32, "groupnorm partials")
+    _need(gamma, torch.float32, "groupnorm gamma")
+    _lib.check(_lib.load().v3d_groupnorm_fold_apply(x.data_ptr(), y.data_ptr(), partials.data_ptr(), gamma.data_ptr(),
+                                                    beta.data_ptr(), rows_per_sample, nsamples, c,
+                                                    c if ldx is None else ldx, groups, nblocks,
+                                                    rows_per_sample if count_rows is None else count_rows, eps,
+                                                    1 if silu else 0, _stream()), "v3d_groupnorm_fold_apply")
+    return y
+
+
+def groupnorm_det_workspace(device, nbytes: int) -> torch.Tensor:
+    """Zeroed workspace of the single-launch deterministic GroupNorm (barrier state + block partials)."""
+    return torch.zeros(nbytes, device=device, dtype=torch.uint8)
+
+
+def groupnorm_det(x: torch.Tensor, y: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, rows_per_sample: int,
+                  hw: int, nsamples: int, c: int, eps: float, silu: bool, workspace: torch.Tensor,
+                  ldx: Optional[int] = None, groups: int = 32) -> torch.Tensor:
+    """groupnorm_partials + groupnorm_fold_apply in one launch (same bits)."""
+    _need(x, torch.bfloat16, "groupnorm x")
+    _need(gamma, torch.float32, "groupnorm gamma")
+    _need(workspace, torch.uint8, "groupnorm workspace")
+    _lib.check(_lib.load().v3d_groupnorm_det(x.data_ptr(), y.data_ptr(), gamma.data_ptr(), beta.data_ptr(),
+                                             rows_per_sample, hw, nsamples, c, c if ldx is None else ldx, groups, eps,
+                                             1 if silu else 0, workspace.data_ptr(), workspace.numel(), _stream()),
+               "v3d_groupnorm_det")
     return y
 
 

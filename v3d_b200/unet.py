@@ -184,8 +184,23 @@ class KernelModule(nn.Module):
             object.__setattr__(self, "_gn_ws", ws)
         return ws
 
+    def _gn_det_workspace(self, dev, nbytes: int) -> torch.Tensor:
+        """Workspace of the single-launch deterministic GroupNorm, sized by shape: one zeroed buffer per power-of-two
+        size class and device.  None is ever freed while the module lives (a captured CUDA graph holds its address)."""
+        pool = getattr(self, "_gn_det_ws", None)
+        if pool is None:
+            pool = {}
+            object.__setattr__(self, "_gn_det_ws", pool)
+        size = 1 << max(int(nbytes) - 1, 1).bit_length()
+        ws = pool.get((dev, size))
+        if ws is None:
+            ws = pool[(dev, size)] = ops.groupnorm_det_workspace(dev, size)
+        return ws
+
     def _gn(self, P: dict, key: str, x: torch.Tensor, rows_per_sample: int, nsamples: int, c: int, eps: float,
-            silu: bool) -> torch.Tensor:
+            silu: bool, hw: Optional[int] = None) -> torch.Tensor:
+        """act(GroupNorm32(x)) over nsamples x rows_per_sample rows; hw = rows per frame (3-D norms: rows_per_sample =
+        T * hw), which defines the blocks of the deterministic statistics."""
         y = torch.empty(x.shape[0], c, device=x.device, dtype=torch.bfloat16)
         # one launch (statistics -> grid barrier -> apply) for the per-frame (2-D) norms: on one H100 it measured faster
         # than the statistics + apply pair at every such UNet shape (tools/microbench.py norm: 0.116 vs 0.139 ms at
@@ -193,6 +208,18 @@ class KernelModule(nn.Module):
         # 604 MB tensors (0.641 vs 0.669 ms); the UNet's largest is 283 MB, so the 300 MB bound excludes none of them.
         # At 1.2 GB the two tie.  The 3-D time_stack norms (2 samples) stay on the pair
         fused = 8 <= nsamples <= 256 and x.numel() * 2 <= 300e6
+        if ops.deterministic():
+            # the same selection between one launch and the pair, on the deterministic kernels (same bits either way)
+            hw = rows_per_sample if hw is None else hw
+            if fused and os.environ.get("V3D_GN_FUSED", "1") != "0":
+                ws = self._gn_det_workspace(x.device, ops.groupnorm_det_workspace_bytes(rows_per_sample, hw, nsamples))
+                return ops.groupnorm_det(x, y, P[key + ".weight"], P[key + ".bias"], rows_per_sample, hw, nsamples, c,
+                                         eps, silu, ws)
+            nblk = ops.groupnorm_det_blocks(rows_per_sample, hw)
+            part = torch.empty(nsamples, nblk, 32, 2, device=x.device, dtype=torch.float32)
+            ops.groupnorm_partials(x, part, rows_per_sample, hw, nsamples, c)
+            return ops.groupnorm_fold_apply(x, y, part, P[key + ".weight"], P[key + ".bias"], rows_per_sample,
+                                            nsamples, c, eps, silu, nblk)
         if fused and os.environ.get("V3D_GN_FUSED", "1") != "0":
             return ops.groupnorm(x, y, P[key + ".weight"], P[key + ".bias"], rows_per_sample, nsamples, c, eps, silu,
                                  self._gn_workspace(x.device))
@@ -208,6 +235,20 @@ class KernelModule(nn.Module):
         the interior of a [nb, tl + 2, hw, c] buffer whose first / last frame then receive the neighbours' boundary
         frames (zeros at the ends of the video): the operand of the following (3,1,1) convolution."""
         vs = self.view_shard
+        if ops.deterministic():
+            # block partials of this rank's frames at their global block offset, all-gathered, folded over the whole
+            # video in block order on every rank: the unsharded deterministic statistics, bit for bit
+            nbf = ops.groupnorm_det_blocks(hw, hw)
+            part = vs.gn_partials(nb, vs.num_frames * nbf, x.device)
+            ops.groupnorm_partials(x, part[:, vs.t0 * nbf:], tl * hw, hw, nb, c, ldp=vs.num_frames * nbf)
+            vs.allgather_partials_(part, nbf)
+            pad = vs.new_pad((nb, tl + 2, hw, c), torch.bfloat16, x.device)
+            for b in range(nb):
+                ops.groupnorm_fold_apply(x[b * tl * hw:(b + 1) * tl * hw], pad[b, 1:tl + 1], part[b:b + 1],
+                                         P[key + ".weight"], P[key + ".bias"], tl * hw, 1, c, eps, silu,
+                                         vs.num_frames * nbf, count_rows=vs.num_frames * hw)
+            vs.exchange_halos(pad)
+            return pad
         stats, pre_zeroed = self._take_stats(nb, x.device)
         ops.groupnorm_stats(x, stats, tl * hw, nb, c, pre_zeroed=pre_zeroed)
         vs.allreduce_stats_(stats)
@@ -716,9 +757,15 @@ class VideoUNet(KernelModule):
         args = (x.float().contiguous(), timesteps.float().contiguous(), ctx2d.contiguous(), y.float().contiguous())
         return args, (B, T, nb, H, W), graphs
 
-    def _run_graphed(self, P, args, B, T, nb, H, W, dev):
+    def _graph_key(self, B, T, H, W, dev) -> tuple:
+        """Cache key of a captured graph: the shape, the device, the shard and the deterministic mode (the two modes
+        launch different GroupNorm kernels, so a graph captured in one is never replayed in the other)."""
         vs = self.view_shard
         key = (B, T, H, W, dev.index) if vs is None else (B, T, H, W, dev.index, vs.num_frames, vs.rank, vs.world)
+        return key + (("deterministic",) if ops.deterministic() else ())
+
+    def _run_graphed(self, P, args, B, T, nb, H, W, dev):
+        key = self._graph_key(B, T, H, W, dev)
         entry = self._graphs.get(key)
         if entry is None:
             # first call with this shape runs eagerly: warms kernel attributes and the positional-embedding cache
@@ -803,11 +850,11 @@ class VideoUNet(KernelModule):
         ts = nm + ".time_stack"
         norm = self._gn_halo if self.view_shard is not None else None
         a = (norm(P, ts + ".in_layers.0", xs, hw, T, nb, cout, 1e-5, True) if norm else
-             self._gn(P, ts + ".in_layers.0", xs, T * hw, nb, cout, 1e-5, True))
+             self._gn(P, ts + ".in_layers.0", xs, T * hw, nb, cout, 1e-5, True, hw=hw))
         h2 = torch.empty(rows, cout, device=x.device, dtype=torch.bfloat16)
         self._tconv(P, ts + ".in_layers.2", a, h2, hw, T, nb, cout, fbias=emb_all[:, o3:], ldfb=E, rows_per_frame=hw)
         a = (norm(P, ts + ".out_layers.0", h2, hw, T, nb, cout, 1e-5, True) if norm else
-             self._gn(P, ts + ".out_layers.0", h2, T * hw, nb, cout, 1e-5, True))
+             self._gn(P, ts + ".out_layers.0", h2, T * hw, nb, cout, 1e-5, True, hw=hw))
         alpha = P[nm + ".alpha"]
         self._tconv(P, ts + ".out_layers.3", a, h2, hw, T, nb, cout, r1=xs, s1=1.0, s0=1.0 - alpha)
         return h2

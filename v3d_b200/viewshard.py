@@ -10,7 +10,8 @@ projections: ~93 % of the UNet's FLOPs).  Three things couple the frames and eac
   * the (3,1,1) temporal convolutions (video_model.py:42-55, temporal_ae.py:94-99): one halo frame from each
     neighbour (`exchange_halos`); the video's first / last frame keep the reference's ZERO padding;
   * the 3-D GroupNorms of the time_stack ResBlocks (openaimodel.py:267-271 with dims=3): (sum, sum of squares)
-    all-reduce of the fp64 statistics (`allreduce_stats_`).
+    all-reduce of the fp64 statistics (`allreduce_stats_`); in deterministic mode an all-gather of the block partials
+    instead (`allgather_partials_`), folded over the whole video in one fixed order on every rank.
 
 The CFG pair [uc; c] of a frame lives on the same rank, so the guidance combine and the Euler update are local.
 Two transports carry the exchanges.  `PeerTransport` (default when the group runs over NCCL, i.e. one GPU per rank
@@ -190,6 +191,33 @@ class PeerTransport:
                                                    self.ctrl.data_ptr(), self.ctrl.data_ptr() + 4, st["id"],
                                                    _stream_of(self.dev)), "v3d_peer_allreduce_f64")
         return stats
+
+    def partials(self, nb: int, nblk: int, groups: int) -> torch.Tensor:
+        """Block-partial buffer [nb, nblk, groups, 2] fp32 of one deterministic 3-D GroupNorm (the whole video's
+        blocks), in the arena; unique per site, like the statistics slots."""
+        nbytes = 8 * nb * nblk * groups
+        st = self._site("partials", (nb, nblk, groups), lambda: {"buf": self._take(nbytes), "flags": self._flags(self.world)})
+        t = self._view(st["buf"], nbytes).view(torch.float32).view(nb, nblk, groups, 2)
+        t._v3d_site = st
+        return t
+
+    def allgather_partials(self, part: torch.Tensor, first_block: int, nblocks: int) -> None:
+        """This rank's blocks [first_block, first_block + nblocks) of every video -> the same place in every other
+        rank's buffer; then wait until every rank's blocks have landed here."""
+        st = part._v3d_site
+        nb, nblk = part.shape[0], part.shape[1]
+        bb = part[0, 0].numel() * part.element_size()                # bytes per block
+        others = [r for r in range(self.world) if r != self.rank]
+        segs = []
+        for r in others:
+            for b in range(nb):
+                off = (b * nblk + first_block) * bb
+                segs.append((self._addr(st["buf"], self.rank, off), self._addr(st["buf"], r, off), nblocks * bb))
+        if len(segs) > 16:
+            raise RuntimeError(f"peer transport: a partials all-gather of {nb} videos over {self.world} ranks needs "
+                               f"{len(segs)} segments (at most 16)")
+        self._put(segs, [self._addr(st["flags"], r, 4 * self.rank) for r in others])
+        self._wait([self._addr(st["flags"], self.rank, 4 * r) for r in others], st["id"])
 
     def pad(self, shape: Tuple[int, ...], cap_shape: Tuple[int, ...], dtype: torch.dtype) -> torch.Tensor:
         """Halo'd operand buffer [nb, tl + 2, ...] living in the arena (capacity for the largest block)."""
@@ -414,6 +442,40 @@ class ViewShard:
                 dist.all_reduce(stats, group=self.group)
         stats.mul_(self.tl / self.num_frames)
         return stats
+
+    def gn_partials(self, nb: int, nblk: int, device, groups: int = 32) -> torch.Tensor:
+        """[nb, nblk, groups, 2] fp32 buffer for the block partials of a deterministic 3-D GroupNorm over the whole
+        video (nblk = all T frames' blocks): plain memory, or - peer transport - arena memory the other ranks write
+        their blocks into"""
+        if self.peer is None:
+            return torch.empty(nb, nblk, groups, 2, device=device, dtype=torch.float32)
+        return self.peer.partials(nb, nblk, groups)
+
+    def allgather_partials_(self, part: torch.Tensor, blocks_per_frame: int) -> torch.Tensor:
+        """Deterministic mode's statistics exchange: part [nb, T * blocks_per_frame, groups, 2] holds this rank's
+        frames' block partials at their global block offset; afterwards it holds every frame's, on every rank."""
+        self._count("gn_allgather")
+        if self.world == 1:
+            return part
+        nbf = blocks_per_frame
+        if self.peer is not None:
+            self.peer.allgather_partials(part, self.t0 * nbf, self.tl * nbf)
+            return part
+        nb = part.shape[0]
+        send = part.new_zeros((nb, self.tmax * nbf) + tuple(part.shape[2:]))   # every rank's slot: the largest block
+        send[:, :self.tl * nbf] = part[:, self.t0 * nbf:(self.t0 + self.tl) * nbf]
+        out = part.new_empty((self.world * send.numel(),))
+        if self._via_host(part):
+            h = torch.empty(out.shape, dtype=out.dtype)
+            dist.all_gather_into_tensor(h, send.reshape(-1).cpu(), group=self.group)
+            out.copy_(h)
+        else:
+            dist.all_gather_into_tensor(out, send.reshape(-1), group=self.group)
+        out = out.view((self.world,) + tuple(send.shape))
+        for r, (t0, n) in enumerate(self.blocks):
+            if r != self.rank:
+                part[:, t0 * nbf:(t0 + n) * nbf] = out[r, :, :n * nbf]
+        return part
 
     def exchange_halos(self, pad: torch.Tensor) -> torch.Tensor:
         """pad: [nb, tl + 2, ...] contiguous; frames 1..tl are this rank's, frame 0 / tl+1 receive the previous /

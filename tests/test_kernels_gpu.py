@@ -491,11 +491,12 @@ def test_heun_step_kernel():
     assert torch.allclose(out, ref, rtol=1e-5, atol=1e-5)
 
 
-@pytest.mark.parametrize("poly", [2])
+@pytest.mark.parametrize("poly", [1, 2, 3])
 def test_attention_poly_exp2_subprocess(poly):
     """FMA-pipe exp2 for 2 / 4 / 6 of a tile's 8 key chunks (V3D_ATTN_POLY, read once per process): the spatial
-    attention tests (random and peaked rows, vs fp32 SDPA and the mma.sync twin) re-run in a child with the switch on.
-    The polynomial's max relative error is 8e-5 (1.5e-4 at 2^-126), far inside those tests' bf16 tolerances."""
+    attention tests (random and peaked rows, vs fp32 SDPA and the mma.sync twin; tail and planted-score cases vs fp64)
+    re-run in a child with the switch on.  The polynomial's max relative error is 8e-5 (1.5e-4 at 2^-126), far inside
+    those tests' bf16 tolerances."""
     import subprocess
     import sys
     from pathlib import Path
@@ -503,8 +504,9 @@ def test_attention_poly_exp2_subprocess(poly):
     here = Path(__file__).resolve().parent
     env = dict(os.environ, V3D_ATTN_POLY=str(poly))
     res = subprocess.run([sys.executable, "-m", "pytest", str(here / "test_kernels_gpu.py"),
-                          str(here / "test_zz_attention_rescale_gpu.py"), "-x", "-q", "-m", "gpu", "-k",
-                          "attention_spatial"], env=env, capture_output=True, text=True, timeout=600)
+                          str(here / "test_zz_attention_rescale_gpu.py"), str(here / "test_kernel_edges_fp64_gpu.py"),
+                          "-x", "-q", "-m", "gpu", "-k", "attention_spatial"], env=env, capture_output=True, text=True,
+                         timeout=600)
     assert res.returncode == 0, res.stdout[-3000:] + res.stderr[-2000:]
 
 

@@ -13,6 +13,7 @@ import torch
 import torch.nn.functional as F
 
 SD = Dict[str, torch.Tensor]
+SDPA_CHUNK_BYTES = 1 << 30      # largest score tensor one attention call materialises
 
 
 @dataclass
@@ -95,8 +96,10 @@ def timestep_embedding(t: torch.Tensor, dim: int, max_period: float = 10000.0) -
 
 
 def group_norm32(x: torch.Tensor, sd: SD, p: str, eps: float) -> torch.Tensor:
-    """GroupNorm32(32, C) eps 1e-5 in fp32 (util.py:259-276) / Normalize eps 1e-6 (attention.py:130-133)."""
-    return F.group_norm(x.float(), 32, sd[p + ".weight"], sd[p + ".bias"], eps).type(x.dtype)
+    """GroupNorm32(32, C) eps 1e-5 in fp32 (util.py:259-276) / Normalize eps 1e-6 (attention.py:130-133).
+    At least fp32: an fp64 input (the block-isolated checks) is normalised in fp64, on the input's device."""
+    dt = torch.promote_types(x.dtype, torch.float32)
+    return F.group_norm(x.to(dt), 32, sd[p + ".weight"].to(dt), sd[p + ".bias"].to(dt), eps).type(x.dtype)
 
 
 def lin(x: torch.Tensor, sd: SD, p: str) -> torch.Tensor:
@@ -110,7 +113,8 @@ def layer_norm(x: torch.Tensor, sd: SD, p: str) -> torch.Tensor:
 def alpha_blend(sd: SD, p: str, x_spatial, x_temporal, indicator: torch.Tensor, pattern: str):
     """AlphaBlender, merge_strategy learned_with_images (util.py:341-369):
     alpha = where(indicator, 1, sigmoid(mix_factor)); alpha*x_spatial + (1-alpha)*x_temporal."""
-    alpha = torch.where(indicator.bool(), torch.ones(1, 1), torch.sigmoid(sd[p + ".mix_factor"])[..., None])
+    mix = torch.sigmoid(sd[p + ".mix_factor"])[..., None]
+    alpha = torch.where(indicator.bool().to(mix.device), torch.ones(1, 1, dtype=mix.dtype, device=mix.device), mix)
     b, t = alpha.shape
     if pattern == "b t -> b 1 t 1 1":
         alpha = alpha.reshape(b, 1, t, 1, 1)
@@ -165,7 +169,16 @@ def attention(sd: SD, p: str, x: torch.Tensor, context: Optional[torch.Tensor], 
     def split(t):
         return t.reshape(b, -1, heads, d).permute(0, 2, 1, 3)
 
-    o = F.scaled_dot_product_attention(split(q), split(k), split(v))
+    q, k, v = split(q), split(k), split(v)
+    # the score matrices of every (sample, head) at once, unless they pass SDPA_CHUNK_BYTES (an fp64 SDPA over
+    # 36 samples x 5 heads x 4096^2 scores is 24 GB): then a few (sample, head) pairs per call
+    step = max(1, SDPA_CHUNK_BYTES // (q.shape[2] * k.shape[2] * q.element_size()))
+    if step >= b * heads:
+        o = F.scaled_dot_product_attention(q, k, v)
+    else:
+        q, k, v = (t.reshape(b * heads, 1, -1, d) for t in (q, k, v))
+        o = torch.cat([F.scaled_dot_product_attention(q[i:i + step], k[i:i + step], v[i:i + step])
+                       for i in range(0, b * heads, step)]).reshape(b, heads, n, d)
     o = o.permute(0, 2, 1, 3).reshape(b, n, c)
     return lin(o, sd, p + ".to_out.0")
 
@@ -207,8 +220,8 @@ def spatial_video_transformer(sd: SD, p: str, x, context, T: int, indicator, hea
     x = group_norm32(x, sd, p + ".norm", 1e-6)
     x = x.permute(0, 2, 3, 1).reshape(bt, h * w, c)
     x = lin(x, sd, p + ".proj_in")
-    frames = torch.arange(T).repeat(bt // T)
-    t_emb = timestep_embedding(frames, c)
+    frames = torch.arange(T, device=x.device).repeat(bt // T)
+    t_emb = timestep_embedding(frames, c).to(x.dtype)          # sinusoids in fp32 like the reference
     emb = lin(F.silu(lin(t_emb, sd, p + ".time_pos_embed.0")), sd, p + ".time_pos_embed.2")[:, None, :]
     x = basic_transformer_block(sd, p + ".transformer_blocks.0", x, context, heads)
     x_mix = video_transformer_block(sd, p + ".time_stack.0", x + emb, time_context, T, heads)
@@ -218,14 +231,20 @@ def spatial_video_transformer(sd: SD, p: str, x, context, T: int, indicator, hea
     return x + x_in
 
 
+def unet_embedding(sd: SD, spec: UNetSpec, timesteps: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
+    """time_embed(timestep_embedding(t)) + label_emb(y) (video_model.py:462-467), in y's dtype; the sinusoids are
+    fp32 like the reference's."""
+    t_emb = timestep_embedding(timesteps, spec.model_channels).to(y.dtype)
+    emb = lin(F.silu(lin(t_emb, sd, "time_embed.0")), sd, "time_embed.2")
+    return emb + lin(F.silu(lin(y, sd, "label_emb.0.0")), sd, "label_emb.0.2")
+
+
 def unet_forward(sd: SD, spec: UNetSpec, x, timesteps, context, y, num_video_frames: int, image_only_indicator,
                  taps: Optional[dict] = None):
     """VideoUNet.forward (video_model.py:442-493). `taps`, if given, receives block outputs by name."""
     T = num_video_frames
-    t_emb = timestep_embedding(timesteps, spec.model_channels)
-    emb = lin(F.silu(lin(t_emb, sd, "time_embed.0")), sd, "time_embed.2")
+    emb = unet_embedding(sd, spec, timesteps, y.to(x.dtype))
     assert y.shape[0] == x.shape[0]
-    emb = emb + lin(F.silu(lin(y, sd, "label_emb.0.0")), sd, "label_emb.0.2")
     h = x
     hs = []
     for name, kind, prm in spec.blocks:

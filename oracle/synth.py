@@ -8,6 +8,7 @@ without shipping a 6 GB state_dict.
 """
 from __future__ import annotations
 
+import math
 import zlib
 from typing import Dict, Iterable, Tuple
 
@@ -56,3 +57,23 @@ def synth_inputs(T: int, latent_hw: int, seed: int = 23, ctx_dim: int = 1024, ad
     c = {"crossattn": cross, "concat": concat, "vector": vector}
     uc = {"crossattn": torch.zeros_like(cross), "concat": torch.zeros_like(concat), "vector": vector.clone()}
     return x, c, uc
+
+
+def synth_inputs_perframe(T: int, latent_hw: int, seed: int = 29, ctx_dim: int = 1024, adm: int = 768):
+    """Conditioning in which every frame and both CFG halves differ, so that a launch reading another frame's or
+    another sample's row changes the numbers: crossattn, concat and vector are drawn per frame and per half (uc is not
+    zero), and every one of the 2T samples gets its own timestep c_noise = log(sigma) / 4, with sigma log-spaced over
+    [0.002, 700] in a seeded order.  -> x [T,4,h,w], c, uc, timesteps [2T] (uc half first, like the guider)."""
+    g = torch.Generator(device="cpu")
+    g.manual_seed(seed)
+    x = torch.randn(T, 4, latent_hw, latent_hw, generator=g)
+
+    def cond():
+        return {"crossattn": torch.randn(T, 1, ctx_dim, generator=g),
+                "concat": torch.randn(T, 4, latent_hw, latent_hw, generator=g),
+                "vector": torch.randn(T, adm, generator=g)}
+
+    c, uc = cond(), cond()
+    sigma = torch.logspace(math.log10(0.002), math.log10(700.0), 2 * T, dtype=torch.float64)
+    timesteps = (0.25 * sigma.log()).float()[torch.randperm(2 * T, generator=g)]
+    return x, c, uc, timesteps

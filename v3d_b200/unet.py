@@ -971,7 +971,9 @@ class VideoUNet(KernelModule):
                 ops.copy_channels(cur, ch, cat, ch + sc, rows, ch)
                 ops.copy_channels(skip, sc, cat[:, ch:], ch + sc, rows, sc)
                 cur, ch = cat, ch + sc
-            if self.debug_taps is not None and st.name in self.debug_taps and st.kind in ("res", "attn", "down", "up"):
+            # a tap is the block's bf16 output widened to fp32 NCHW: exactly the next block's input
+            if self.debug_taps is not None and st.name in self.debug_taps and st.kind in ("conv_in", "res", "attn",
+                                                                                          "down", "up"):
                 tap = torch.empty(B, ch, h, w, device=dev, dtype=torch.float32)
                 ops.nhwc_to_nchw_f32(cur, tap, B, ch, h * w, ch)
                 self.debug_taps[st.name] = tap

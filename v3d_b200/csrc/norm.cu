@@ -10,376 +10,77 @@
 namespace v3d {
 
 // ------------------------------------------------------------------------------------------------
-// GroupNorm statistics: stats[sample][group] = {sum, sumsq} (double), accumulated with atomics.
-// grid = (row chunks, samples); each thread owns one 8-channel vector column and strides over rows.
+// GroupNorm over [samples][rows][C] bf16 (row stride ldx) -> y dense, act = optional SiLU.
+// Every kernel uses one thread layout: thread t owns the 8-channel vector column vc = t % vpr (vpr = C / 8) and the
+// row lane rl = t / vpr of lanes_r = blockDim.x / vpr; over rows [r0, r1) it visits r0 + rl, r0 + rl + lanes_r, ...
+//
+// Statistics blocks: a sample's rows, [frames][hw], are cut into blocks of R rows that never straddle a frame (the
+// last block of a frame may be short).  Each (block, group) gets ONE fp32 (sum, sumsq) pair from a fixed in-CTA tree,
+// and a sample's pairs are folded in fp64 in block order.  No atomics on data, so the result depends only on the block
+// geometry and the data:
+//   default mode        one block per CTA (hw = rows_per_sample, R = rows per CTA, chosen from the co-resident grid);
+//   deterministic mode  R = min(256, hw), whatever the grid, nsamples or sharded plan (the partials of a frame subset
+//                       equal those of the same frames inside the whole tensor), so the partials + fold_apply pair,
+//                       the single launch and every sharded plan produce the same bits.
+// gn_stats_kernel alone sums with atomics (fp64 out, all-reduced by the frame-sharded default path).
 // ------------------------------------------------------------------------------------------------
 constexpr int kGnThreads = 256;
 constexpr int kGnUnroll = 8;  // independent 16-byte loads in flight per thread
-
-__global__ void __launch_bounds__(512)
-gn_stats_kernel(const bf16* __restrict__ x, double* __restrict__ stats, long long rows_per_sample,
-                int C, long long ldx, int groups, int rows_per_cta) {
-  extern __shared__ float s_acc[];  // [2][C]
-  const int vpr = C >> 3;           // 16-byte vectors per row
-  const int sample = blockIdx.y;
-  const long long row0 = static_cast<long long>(blockIdx.x) * rows_per_cta;
-  long long row1 = row0 + rows_per_cta;
-  if (row1 > rows_per_sample) row1 = rows_per_sample;
-  for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) s_acc[i] = 0.f;
-  __syncthreads();
-
-  const int lanes_r = blockDim.x / vpr;  // row lanes (block = vpr * lanes_r threads)
-  const int vc = threadIdx.x % vpr;
-  const int rl = threadIdx.x / vpr;
-  float s[8], q[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) s[j] = q[j] = 0.f;
-  const bf16* base = x + (static_cast<long long>(sample) * rows_per_sample) * ldx + vc * 8;
-  long long r = row0 + rl;
-  for (; r + static_cast<long long>(kGnUnroll - 1) * lanes_r < row1; r += static_cast<long long>(kGnUnroll) * lanes_r) {
-    uint4 u[kGnUnroll];
-#pragma unroll
-    for (int k = 0; k < kGnUnroll; ++k)
-      u[k] = __ldg(reinterpret_cast<const uint4*>(base + (r + static_cast<long long>(k) * lanes_r) * ldx));
-#pragma unroll
-    for (int k = 0; k < kGnUnroll; ++k) {
-      const uint32_t w[4] = {u[k].x, u[k].y, u[k].z, u[k].w};
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 f = unpack_bf16x2(w[j]);
-        s[2 * j] += f.x; q[2 * j] = fmaf(f.x, f.x, q[2 * j]);
-        s[2 * j + 1] += f.y; q[2 * j + 1] = fmaf(f.y, f.y, q[2 * j + 1]);
-      }
-    }
-  }
-  for (; r < row1; r += lanes_r) {
-    const uint4 u = __ldg(reinterpret_cast<const uint4*>(base + r * ldx));
-    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 f = unpack_bf16x2(w[j]);
-      s[2 * j] += f.x; q[2 * j] = fmaf(f.x, f.x, q[2 * j]);
-      s[2 * j + 1] += f.y; q[2 * j + 1] = fmaf(f.y, f.y, q[2 * j + 1]);
-    }
-  }
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    atomicAdd(&s_acc[vc * 8 + j], s[j]);
-    atomicAdd(&s_acc[C + vc * 8 + j], q[j]);
-  }
-  __syncthreads();
-  const int cg = C / groups;
-  for (int g = threadIdx.x; g < groups; g += blockDim.x) {
-    double ds = 0.0, dq = 0.0;
-    for (int c = 0; c < cg; ++c) {
-      ds += static_cast<double>(s_acc[g * cg + c]);
-      dq += static_cast<double>(s_acc[C + g * cg + c]);
-    }
-    double* o = stats + (static_cast<long long>(sample) * groups + g) * 2;
-    atomicAdd(o, ds);
-    atomicAdd(o + 1, dq);
-  }
-}
-
-// y = act((x - mean) * rstd * gamma + beta). Each thread owns one 8-channel vector column: its scale/shift
-// (16 floats) are computed once from the statistics and kept in registers; no smem, no div/mod in the loop.
-__global__ void __launch_bounds__(512)
-gn_apply_kernel(const bf16* __restrict__ x, bf16* __restrict__ y, const double* __restrict__ stats,
-                const float* __restrict__ gamma, const float* __restrict__ beta,
-                long long rows_per_sample, int C, long long ldx, int groups, float eps, int silu,
-                int rows_per_cta) {
-  const int vpr = C >> 3;
-  const int sample = blockIdx.y;
-  const int lanes_r = blockDim.x / vpr;
-  const int vc = threadIdx.x % vpr;
-  const int rl = threadIdx.x / vpr;
-  const int cg = C / groups;
-  const double cnt = static_cast<double>(rows_per_sample) * cg;
-  float sc[8], sh[8];
-  {
-    int g_prev = -1;
-    float mean_f = 0.f, rstd_f = 0.f;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int c = vc * 8 + j;
-      const int g = c / cg;
-      if (g != g_prev) {
-        const double* st = stats + (static_cast<long long>(sample) * groups + g) * 2;
-        const double mean = st[0] / cnt;
-        double var = st[1] / cnt - mean * mean;
-        if (var < 0.0) var = 0.0;
-        mean_f = static_cast<float>(mean);
-        rstd_f = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
-        g_prev = g;
-      }
-      const float a = rstd_f * __ldg(gamma + c);
-      sc[j] = a;
-      sh[j] = __ldg(beta + c) - mean_f * a;
-    }
-  }
-  const long long row0 = static_cast<long long>(blockIdx.x) * rows_per_cta;
-  long long row1 = row0 + rows_per_cta;
-  if (row1 > rows_per_sample) row1 = rows_per_sample;
-  const long long srow = static_cast<long long>(sample) * rows_per_sample;
-  const bf16* xb = x + srow * ldx + vc * 8;
-  bf16* yb = y + srow * static_cast<long long>(C) + vc * 8;
-
-  auto emit = [&](const uint4& u, long long r) {
-    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-    uint32_t o[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 f = unpack_bf16x2(w[j]);
-      float a = fmaf(f.x, sc[2 * j], sh[2 * j]);
-      float b = fmaf(f.y, sc[2 * j + 1], sh[2 * j + 1]);
-      if (silu) {
-        a = silu_f(a);
-        b = silu_f(b);
-      }
-      o[j] = pack_bf16x2(a, b);
-    }
-    *reinterpret_cast<uint4*>(yb + r * static_cast<long long>(C)) = make_uint4(o[0], o[1], o[2], o[3]);
-  };
-  long long r = row0 + rl;
-  for (; r + static_cast<long long>(kGnUnroll - 1) * lanes_r < row1; r += static_cast<long long>(kGnUnroll) * lanes_r) {
-    uint4 u[kGnUnroll];
-#pragma unroll
-    for (int k = 0; k < kGnUnroll; ++k)
-      u[k] = __ldg(reinterpret_cast<const uint4*>(xb + (r + static_cast<long long>(k) * lanes_r) * ldx));
-#pragma unroll
-    for (int k = 0; k < kGnUnroll; ++k) emit(u[k], r + static_cast<long long>(k) * lanes_r);
-  }
-  for (; r < row1; r += lanes_r) emit(__ldg(reinterpret_cast<const uint4*>(xb + r * ldx)), r);
-}
-
-// ------------------------------------------------------------------------------------------------
-// GroupNorm in ONE launch: statistics, a grid-wide barrier, then the normalisation of the same rows.
-//   phase 1  every thread sums (x, x^2) of its 8-channel column over its rows; the CTA folds its threads' partials per
-//            group through shared memory + a warp-shuffle tree and writes ONE fp32 (sum, sumsq) pair per group;
-//   barrier  sense-reversing counter in the workspace; the grid is sized to be co-resident (occupancy x SMs);
-//   phase 2  every CTA adds the partials of its sample in fp64, chunk order fixed by the launch geometry (warp-shuffle
-//            tree again) -> mean / rstd, then re-reads its rows in REVERSE order (the rows read last are the ones most
-//            likely still in the 50 MB L2) and writes act((x - mean) rstd gamma + beta).
-// No atomics on data: the result is bit-reproducible run to run.  One launch and one HBM read less than the
-// stats + apply pair, which stays for the frame-sharded path (statistics all-reduce between the two).
-// ------------------------------------------------------------------------------------------------
-struct GnBarrier {
-  unsigned int count;
-  unsigned int gen;
-};
-constexpr int kGnMaxCtas = 4096;                                   // partial slots in the workspace
-constexpr size_t kGnWsBytes = 256 + sizeof(float) * 2 * 32 * kGnMaxCtas;
-
-__device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int* p) {
-  unsigned int v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void st_release_u32(unsigned int* p, unsigned int v) {
-  asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ double warp_sum_f64(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-// MAXT / MINB: launch bounds.  <256, 3> (80 registers) is what every width up to C = 2048 uses: three 240-256-thread
-// CTAs per SM instead of two keep enough loads in flight for the streaming phases; wider rows take <512, 1>.
-template <int MAXT, int MINB>
-__global__ void __launch_bounds__(MAXT, MINB)
-gn_fused_kernel(const bf16* __restrict__ x, bf16* __restrict__ y, const float* __restrict__ gamma,
-                const float* __restrict__ beta, GnBarrier* __restrict__ bar, float2* __restrict__ partial,
-                long long rows_per_sample, int C, long long ldx, int groups, float eps, int silu, int rows_per_cta) {
-  extern __shared__ float s_red[];  // [2][lanes_r][C] thread partials, reused as [groups][2] mean / rstd
-  const int vpr = C >> 3;
-  const int sample = blockIdx.y;
-  const int chunks = gridDim.x;
-  const int lanes_r = blockDim.x / vpr;
-  const int vc = threadIdx.x % vpr;
-  const int rl = threadIdx.x / vpr;
-  const int cg = C / groups;
-  // only FULL warps take part in the shuffle trees (240-thread CTAs end in a 16-lane warp: a full-mask shuffle there
-  // would read lanes that do not exist); a trailing partial warp gets warp id >= nwarps and skips those loops
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-  const long long row0 = static_cast<long long>(blockIdx.x) * rows_per_cta;
-  long long row1 = row0 + rows_per_cta;
-  if (row1 > rows_per_sample) row1 = rows_per_sample;
-  const long long srow = static_cast<long long>(sample) * rows_per_sample;
-  const bf16* xb = x + srow * ldx + vc * 8;
-
-  // ---- phase 1: thread partials
-  float s[8], q[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) s[j] = q[j] = 0.f;
-  auto accum = [&](const uint4& u) {
-    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 f = unpack_bf16x2(w[j]);
-      s[2 * j] += f.x; q[2 * j] = fmaf(f.x, f.x, q[2 * j]);
-      s[2 * j + 1] += f.y; q[2 * j + 1] = fmaf(f.y, f.y, q[2 * j + 1]);
-    }
-  };
-  long long r = row0 + rl;
-  for (; r + static_cast<long long>(kGnUnroll - 1) * lanes_r < row1; r += static_cast<long long>(kGnUnroll) * lanes_r) {
-    uint4 u[kGnUnroll];
-#pragma unroll
-    for (int k = 0; k < kGnUnroll; ++k)
-      u[k] = __ldg(reinterpret_cast<const uint4*>(xb + (r + static_cast<long long>(k) * lanes_r) * ldx));
-#pragma unroll
-    for (int k = 0; k < kGnUnroll; ++k) accum(u[k]);
-  }
-  for (; r < row1; r += lanes_r) accum(__ldg(reinterpret_cast<const uint4*>(xb + r * ldx)));
-  {
-    float* ss = s_red + (static_cast<size_t>(rl) * C + vc * 8);
-    float* qq = ss + static_cast<size_t>(lanes_r) * C;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      ss[j] = s[j];
-      qq[j] = q[j];
-    }
-  }
-  __syncthreads();
-  // CTA partial of group g = sum over its cg channels x lanes_r row lanes: one warp per group, shuffle tree
-  const int cta_id = sample * chunks + blockIdx.x;
-  for (int g = warp < nwarps ? warp : groups; g < groups; g += nwarps) {
-    float a = 0.f, b = 0.f;
-    const int n = cg * lanes_r;
-    for (int i = lane; i < n; i += 32) {
-      const int rr = i / cg, cc = g * cg + (i - rr * cg);
-      a += s_red[static_cast<size_t>(rr) * C + cc];
-      b += s_red[static_cast<size_t>(lanes_r + rr) * C + cc];
-    }
-    a = warp_sum(a);
-    b = warp_sum(b);
-    if (lane == 0) partial[static_cast<size_t>(cta_id) * groups + g] = make_float2(a, b);
-  }
-  // ---- grid-wide barrier (sense reversal: works for any grid size launch after launch on one stream)
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    const unsigned int total = gridDim.x * gridDim.y;
-    const unsigned int my_gen = ld_acquire_u32(&bar->gen);
-    __threadfence();
-    const unsigned int prev = atomicAdd(&bar->count, 1u);
-    if (prev == total - 1) {
-      bar->count = 0;
-      __threadfence();
-      st_release_u32(&bar->gen, my_gen + 1);
-    } else {
-      while (ld_acquire_u32(&bar->gen) == my_gen) __nanosleep(64);
-    }
-  }
-  __syncthreads();
-  // ---- phase 2: mean / rstd of this sample's groups (fp64, fixed chunk order), then normalise
-  float* s_stat = s_red;  // [groups][2]
-  const double cnt = static_cast<double>(rows_per_sample) * cg;
-  for (int g = warp < nwarps ? warp : groups; g < groups; g += nwarps) {
-    double a = 0.0, b = 0.0;
-    for (int k = lane; k < chunks; k += 32) {
-      const float2 p = __ldcg(&partial[static_cast<size_t>(sample * chunks + k) * groups + g]);
-      a += static_cast<double>(p.x);
-      b += static_cast<double>(p.y);
-    }
-    a = warp_sum_f64(a);
-    b = warp_sum_f64(b);
-    if (lane == 0) {
-      const double mean = a / cnt;
-      double var = b / cnt - mean * mean;
-      if (var < 0.0) var = 0.0;
-      s_stat[2 * g] = static_cast<float>(mean);
-      s_stat[2 * g + 1] = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
-    }
-  }
-  __syncthreads();
-  float sc[8], sh[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const int c = vc * 8 + j;
-    const int g = c / cg;
-    const float a = s_stat[2 * g + 1] * __ldg(gamma + c);
-    sc[j] = a;
-    sh[j] = __ldg(beta + c) - s_stat[2 * g] * a;
-  }
-  bf16* yb = y + srow * static_cast<long long>(C) + vc * 8;
-  auto emit = [&](const uint4& u, long long rr) {
-    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-    uint32_t o[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 f = unpack_bf16x2(w[j]);
-      float a = fmaf(f.x, sc[2 * j], sh[2 * j]);
-      float b = fmaf(f.y, sc[2 * j + 1], sh[2 * j + 1]);
-      if (silu) {
-        a = silu_f(a);
-        b = silu_f(b);
-      }
-      o[j] = pack_bf16x2(a, b);
-    }
-    *reinterpret_cast<uint4*>(yb + rr * static_cast<long long>(C)) = make_uint4(o[0], o[1], o[2], o[3]);
-  };
-  // reverse order: this thread's rows are row0 + rl + i * lanes_r, i = 0 .. n_i - 1
-  const long long span = row1 - row0 - rl;
-  long long n_i = span > 0 ? (span + lanes_r - 1) / lanes_r : 0;
-  long long i = n_i;
-  for (; i >= kGnUnroll; i -= kGnUnroll) {
-    uint4 u[kGnUnroll];
-#pragma unroll
-    for (int k = 0; k < kGnUnroll; ++k)
-      u[k] = __ldg(reinterpret_cast<const uint4*>(xb + (row0 + rl + (i - 1 - k) * lanes_r) * ldx));
-#pragma unroll
-    for (int k = 0; k < kGnUnroll; ++k) emit(u[k], row0 + rl + (i - 1 - k) * lanes_r);
-  }
-  for (; i > 0; --i) {
-    const long long rr = row0 + rl + (i - 1) * lanes_r;
-    emit(__ldg(reinterpret_cast<const uint4*>(xb + rr * ldx)), rr);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Deterministic GroupNorm (opt-in).  ONE definition of the statistics, whatever the launch geometry:
-//   blocks   a sample's rows, [frames][hw], are cut into blocks of R = min(256, hw) rows; a block never straddles a
-//            frame and the last block of a frame may be short (nbf = ceil(hw / R) blocks per frame);
-//   partial  each (block, group) gets ONE fp32 (sum, sumsq) pair from a fixed in-CTA tree: every thread sums its
-//            8-channel column over the block's rows in row order, then one warp per group adds the group's
-//            (channel, row lane) sums lane-strided and folds the lanes with an xor-shuffle tree;
-//   fold     per (sample, group), in fp64: lane l of one warp adds blocks l, l + 32, l + 64, ... in turn, then an
-//            xor-shuffle tree folds the 32 lanes.
-// The statistics depend on the shape and the data only - not on the grid, on nsamples, on a CFG split or on which rank
-// computed which frames (the partials of a frame subset equal those of the same frames inside the whole tensor), so
-// the two-kernel form, the single-launch form and every sharded plan produce the same bits.
-// ------------------------------------------------------------------------------------------------
 constexpr long long kGnDetRows = 256;
 
 __host__ __device__ __forceinline__ long long gn_det_block_rows(long long hw) { return hw < kGnDetRows ? hw : kGnDetRows; }
-__host__ __device__ __forceinline__ long long gn_det_blocks_per_frame(long long hw) {
-  const long long r = gn_det_block_rows(hw);
-  return (hw + r - 1) / r;
-}
-// rows [r0, r1) of block `blk` of a sample
-__device__ __forceinline__ void gn_det_block_range(long long blk, long long hw, long long& r0, long long& r1) {
-  const long long nbf = gn_det_blocks_per_frame(hw), R = gn_det_block_rows(hw);
-  const long long f = blk / nbf, b = blk - f * nbf;
+__host__ __device__ __forceinline__ long long gn_blocks_per_frame(long long hw, long long R) { return (hw + R - 1) / R; }
+
+// rows [r0, r1) of block `blk` of a sample (frames of hw rows, blocks of R rows); ONE_FRAME: the sample is one frame
+template <bool ONE_FRAME = false>
+__device__ __forceinline__ void gn_block_range(long long blk, long long hw, long long R, long long& r0, long long& r1) {
+  const long long nbf = gn_blocks_per_frame(hw, R);
+  const long long f = ONE_FRAME ? 0 : blk / nbf, b = blk - f * nbf;
   r0 = f * hw + b * R;
   r1 = r0 + R < (f + 1) * hw ? r0 + R : (f + 1) * hw;
 }
 
-// (sum, sumsq) of rows [r0, r1) of one sample (xs = its first row) for every group -> part[g].  Called by every
-// thread of the CTA (it synchronises); s_red = [2][lanes_r][C] floats.
-__device__ __forceinline__ void gn_det_block_partial(const bf16* __restrict__ xs, long long r0, long long r1,
-                                                     long long ldx, int C, int groups, float* s_red,
-                                                     float2* __restrict__ part) {
-  const int vpr = C >> 3;
-  const int lanes_r = blockDim.x / vpr;
-  const int vc = threadIdx.x % vpr;
-  const int rl = threadIdx.x / vpr;
-  const int cg = C / groups;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-  const bf16* xb = xs + vc * 8;
-  float s[8], q[8];
+// f(u, r) for this thread's rows r of [r0, r1) (u = its 16-byte vector of row r; xb = the sample's first row + its
+// column), kGnUnroll loads in flight; ascending rows, or descending when REVERSE.
+template <bool REVERSE, class F>
+__device__ __forceinline__ void gn_rows(const bf16* __restrict__ xb, long long r0, long long r1, long long ldx,
+                                        int lanes_r, int rl, F&& f) {
+  if (!REVERSE) {
+    long long r = r0 + rl;
+    for (; r + static_cast<long long>(kGnUnroll - 1) * lanes_r < r1; r += static_cast<long long>(kGnUnroll) * lanes_r) {
+      uint4 u[kGnUnroll];
+#pragma unroll
+      for (int k = 0; k < kGnUnroll; ++k)
+        u[k] = __ldg(reinterpret_cast<const uint4*>(xb + (r + static_cast<long long>(k) * lanes_r) * ldx));
+#pragma unroll
+      for (int k = 0; k < kGnUnroll; ++k) f(u[k], r + static_cast<long long>(k) * lanes_r);
+    }
+    for (; r < r1; r += lanes_r) f(__ldg(reinterpret_cast<const uint4*>(xb + r * ldx)), r);
+  } else {
+    // this thread's rows are r0 + rl + i * lanes_r, i = 0 .. n_i - 1
+    const long long span = r1 - r0 - rl;
+    long long i = span > 0 ? (span + lanes_r - 1) / lanes_r : 0;
+    for (; i >= kGnUnroll; i -= kGnUnroll) {
+      uint4 u[kGnUnroll];
+#pragma unroll
+      for (int k = 0; k < kGnUnroll; ++k)
+        u[k] = __ldg(reinterpret_cast<const uint4*>(xb + (r0 + rl + (i - 1 - k) * lanes_r) * ldx));
+#pragma unroll
+      for (int k = 0; k < kGnUnroll; ++k) f(u[k], r0 + rl + (i - 1 - k) * lanes_r);
+    }
+    for (; i > 0; --i) {
+      const long long r = r0 + rl + (i - 1) * lanes_r;
+      f(__ldg(reinterpret_cast<const uint4*>(xb + r * ldx)), r);
+    }
+  }
+}
+
+// this thread's column sums (x, x^2) of its 8 channels over its rows of [r0, r1), in row order
+__device__ __forceinline__ void gn_col_sums(const bf16* __restrict__ xb, long long r0, long long r1, long long ldx,
+                                            int lanes_r, int rl, float (&s)[8], float (&q)[8]) {
 #pragma unroll
   for (int j = 0; j < 8; ++j) s[j] = q[j] = 0.f;
-  auto accum = [&](const uint4& u) {
+  gn_rows<false>(xb, r0, r1, ldx, lanes_r, rl, [&](const uint4& u, long long) {
     const uint32_t w[4] = {u.x, u.y, u.z, u.w};
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -387,18 +88,22 @@ __device__ __forceinline__ void gn_det_block_partial(const bf16* __restrict__ xs
       s[2 * j] += f.x; q[2 * j] = fmaf(f.x, f.x, q[2 * j]);
       s[2 * j + 1] += f.y; q[2 * j + 1] = fmaf(f.y, f.y, q[2 * j + 1]);
     }
-  };
-  long long r = r0 + rl;
-  for (; r + static_cast<long long>(kGnUnroll - 1) * lanes_r < r1; r += static_cast<long long>(kGnUnroll) * lanes_r) {
-    uint4 u[kGnUnroll];
-#pragma unroll
-    for (int k = 0; k < kGnUnroll; ++k)
-      u[k] = __ldg(reinterpret_cast<const uint4*>(xb + (r + static_cast<long long>(k) * lanes_r) * ldx));
-#pragma unroll
-    for (int k = 0; k < kGnUnroll; ++k) accum(u[k]);
-  }
-  for (; r < r1; r += lanes_r) accum(__ldg(reinterpret_cast<const uint4*>(xb + r * ldx)));
-  __syncthreads();  // the previous block's tree may still be reading s_red
+  });
+}
+
+// The CTA's column sums -> ONE (sum, sumsq) pair per group in part[g]: through s_red ([2][lanes_r][C] floats), then
+// one warp per group adds the group's (row lane, channel) sums lane-strided and folds the lanes with an xor-shuffle
+// tree.  Only FULL warps take part (240-thread CTAs end in a 16-lane warp: a full-mask shuffle there would read lanes
+// that do not exist).  Called by every thread; the first sync lets a previous call's tree finish reading s_red.
+__device__ __forceinline__ void gn_cta_pairs(const float (&s)[8], const float (&q)[8], int C, int groups, float* s_red,
+                                             float2* __restrict__ part) {
+  const int vpr = C >> 3;
+  const int lanes_r = blockDim.x / vpr;
+  const int vc = threadIdx.x % vpr;
+  const int rl = threadIdx.x / vpr;
+  const int cg = C / groups;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+  __syncthreads();
   {
     float* ss = s_red + (static_cast<size_t>(rl) * C + vc * 8);
     float* qq = ss + static_cast<size_t>(lanes_r) * C;
@@ -423,10 +128,26 @@ __device__ __forceinline__ void gn_det_block_partial(const bf16* __restrict__ xs
   }
 }
 
-// mean / rstd of every group of one sample from its nblk block partials ([nblk][groups]) -> s_stat[groups][2].
-// One warp per group; the fold order depends on nblk only.  The caller synchronises before reading s_stat.
-__device__ __forceinline__ void gn_det_fold(const float2* __restrict__ part, long long nblk, int groups, double cnt,
-                                            float eps, float* s_stat) {
+// s_stat[g] = {mean, rstd} (fp32) of group g from its fp64 (sum, sumsq) over cnt elements
+__device__ __forceinline__ void gn_set_stat(float* s_stat, int g, double sum, double sumsq, double cnt, float eps) {
+  const double mean = sum / cnt;
+  double var = sumsq / cnt - mean * mean;
+  if (var < 0.0) var = 0.0;
+  s_stat[2 * g] = static_cast<float>(mean);
+  s_stat[2 * g + 1] = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
+}
+
+__device__ __forceinline__ double warp_sum_f64(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// mean / rstd of every group of one sample from its nblk block pairs ([nblk][groups]) -> s_stat: one full warp per
+// group, lane l adds blocks l, l + 32, ... in fp64, then an xor-shuffle tree.  The order depends on nblk only.  The
+// caller synchronises before reading s_stat.
+__device__ __forceinline__ void gn_fold(const float2* __restrict__ part, long long nblk, int groups, double cnt,
+                                        float eps, float* s_stat) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
   for (int g = warp < nwarps ? warp : groups; g < groups; g += nwarps) {
     double a = 0.0, b = 0.0;
@@ -437,24 +158,32 @@ __device__ __forceinline__ void gn_det_fold(const float2* __restrict__ part, lon
     }
     a = warp_sum_f64(a);
     b = warp_sum_f64(b);
-    if (lane == 0) {
-      const double mean = a / cnt;
-      double var = b / cnt - mean * mean;
-      if (var < 0.0) var = 0.0;
-      s_stat[2 * g] = static_cast<float>(mean);
-      s_stat[2 * g + 1] = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
-    }
+    if (lane == 0) gn_set_stat(s_stat, g, a, b, cnt, eps);
   }
 }
 
-// y rows [r0, r1) = act(x * sc + sh) for this thread's 8-channel column (xb / yb: the sample's first row + column)
-__device__ __forceinline__ void gn_det_apply_rows(const bf16* __restrict__ xb, bf16* __restrict__ yb, long long r0,
-                                                  long long r1, long long ldx, int C, const float* sc, const float* sh,
-                                                  int silu) {
-  const int vpr = C >> 3;
-  const int lanes_r = blockDim.x / vpr;
-  const int rl = threadIdx.x / vpr;
-  auto emit = [&](const uint4& u, long long rr) {
+// this thread's scale / shift of its 8 channels from s_stat, gamma and beta
+__device__ __forceinline__ void gn_scale_shift(const float* s_stat, const float* __restrict__ gamma,
+                                               const float* __restrict__ beta, int C, int groups, float (&sc)[8],
+                                               float (&sh)[8]) {
+  const int vc = threadIdx.x % (C >> 3);
+  const int cg = C / groups;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int c = vc * 8 + j;
+    const int g = c / cg;
+    const float a = s_stat[2 * g + 1] * __ldg(gamma + c);
+    sc[j] = a;
+    sh[j] = __ldg(beta + c) - s_stat[2 * g] * a;
+  }
+}
+
+// y = act(x * sc + sh) over this thread's rows of [r0, r1) (xb / yb: the sample's first row + this thread's column)
+template <bool REVERSE>
+__device__ __forceinline__ void gn_apply_rows(const bf16* __restrict__ xb, bf16* __restrict__ yb, long long r0,
+                                              long long r1, long long ldx, int C, int lanes_r, int rl,
+                                              const float (&sc)[8], const float (&sh)[8], int silu) {
+  gn_rows<REVERSE>(xb, r0, r1, ldx, lanes_r, rl, [&](const uint4& u, long long r) {
     const uint32_t w[4] = {u.x, u.y, u.z, u.w};
     uint32_t o[4];
 #pragma unroll
@@ -468,90 +197,27 @@ __device__ __forceinline__ void gn_det_apply_rows(const bf16* __restrict__ xb, b
       }
       o[j] = pack_bf16x2(a, b);
     }
-    *reinterpret_cast<uint4*>(yb + rr * static_cast<long long>(C)) = make_uint4(o[0], o[1], o[2], o[3]);
-  };
-  long long r = r0 + rl;
-  for (; r + static_cast<long long>(kGnUnroll - 1) * lanes_r < r1; r += static_cast<long long>(kGnUnroll) * lanes_r) {
-    uint4 u[kGnUnroll];
-#pragma unroll
-    for (int k = 0; k < kGnUnroll; ++k)
-      u[k] = __ldg(reinterpret_cast<const uint4*>(xb + (r + static_cast<long long>(k) * lanes_r) * ldx));
-#pragma unroll
-    for (int k = 0; k < kGnUnroll; ++k) emit(u[k], r + static_cast<long long>(k) * lanes_r);
-  }
-  for (; r < r1; r += lanes_r) emit(__ldg(reinterpret_cast<const uint4*>(xb + r * ldx)), r);
+    *reinterpret_cast<uint4*>(yb + r * static_cast<long long>(C)) = make_uint4(o[0], o[1], o[2], o[3]);
+  });
 }
 
-// per-thread scale / shift of its 8 channels from s_stat
-__device__ __forceinline__ void gn_det_scale_shift(const float* s_stat, const float* __restrict__ gamma,
-                                                   const float* __restrict__ beta, int C, int groups, float* sc,
-                                                   float* sh) {
-  const int vc = threadIdx.x % (C >> 3);
-  const int cg = C / groups;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const int c = vc * 8 + j;
-    const int g = c / cg;
-    const float a = s_stat[2 * g + 1] * __ldg(gamma + c);
-    sc[j] = a;
-    sh[j] = __ldg(beta + c) - s_stat[2 * g] * a;
-  }
+// Sense-reversing grid barrier in the workspace: works for any grid size, launch after launch on one stream, provided
+// every CTA of the grid is resident at once.
+struct GnBarrier {
+  unsigned int count;
+  unsigned int gen;
+};
+
+__device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int* p) {
+  unsigned int v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_release_u32(unsigned int* p, unsigned int v) {
+  asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
-// grid = (blocks per sample, samples): one CTA per block
-__global__ void __launch_bounds__(512)
-gn_det_partials_kernel(const bf16* __restrict__ x, float2* __restrict__ partial, long long rows_per_sample,
-                       long long hw, int C, long long ldx, int groups, long long ldp) {
-  extern __shared__ float s_red[];  // [2][lanes_r][C]
-  const int sample = blockIdx.y;
-  long long r0, r1;
-  gn_det_block_range(blockIdx.x, hw, r0, r1);
-  gn_det_block_partial(x + static_cast<long long>(sample) * rows_per_sample * ldx, r0, r1, ldx, C, groups, s_red,
-                       partial + (static_cast<long long>(sample) * ldp + blockIdx.x) * groups);
-}
-
-// grid = (row chunks, samples): every CTA folds its sample's partials, then normalises its rows
-__global__ void __launch_bounds__(512)
-gn_det_apply_kernel(const bf16* __restrict__ x, bf16* __restrict__ y, const float2* __restrict__ partial,
-                    const float* __restrict__ gamma, const float* __restrict__ beta, long long rows_per_sample, int C,
-                    long long ldx, int groups, long long nblk, long long count_rows, float eps, int silu,
-                    int rows_per_cta) {
-  __shared__ float s_stat[64];  // [groups <= 32][2]
-  const int sample = blockIdx.y;
-  gn_det_fold(partial + static_cast<long long>(sample) * nblk * groups, nblk, groups,
-              static_cast<double>(count_rows) * (C / groups), eps, s_stat);
-  __syncthreads();
-  float sc[8], sh[8];
-  gn_det_scale_shift(s_stat, gamma, beta, C, groups, sc, sh);
-  const long long row0 = static_cast<long long>(blockIdx.x) * rows_per_cta;
-  long long row1 = row0 + rows_per_cta;
-  if (row1 > rows_per_sample) row1 = rows_per_sample;
-  const long long srow = static_cast<long long>(sample) * rows_per_sample;
-  const int vc = threadIdx.x % (C >> 3);
-  gn_det_apply_rows(x + srow * ldx + vc * 8, y + srow * static_cast<long long>(C) + vc * 8, row0, row1, ldx, C, sc, sh,
-                    silu);
-}
-
-// Single launch, deterministic: the CTAs of a sample stride over its blocks (CTA i takes blocks i, i + gridDim.x, ...)
-// and write the block partials, a grid-wide barrier, then EVERY CTA folds all blocks of its sample (so the fold does
-// not depend on gridDim) and normalises the rows of its own blocks, last block first (the rows read last are the ones
-// most likely still in L2).
-template <int MAXT, int MINB>
-__global__ void __launch_bounds__(MAXT, MINB)
-gn_det_fused_kernel(const bf16* __restrict__ x, bf16* __restrict__ y, const float* __restrict__ gamma,
-                    const float* __restrict__ beta, GnBarrier* __restrict__ bar, float2* __restrict__ partial,
-                    long long rows_per_sample, long long hw, int C, long long ldx, int groups, float eps, int silu) {
-  extern __shared__ float s_red[];  // [2][lanes_r][C] thread partials, reused as [groups][2] mean / rstd
-  const int sample = blockIdx.y;
-  const long long nblk = rows_per_sample / hw * gn_det_blocks_per_frame(hw);
-  const bf16* xs = x + static_cast<long long>(sample) * rows_per_sample * ldx;
-  float2* ps = partial + static_cast<long long>(sample) * nblk * groups;
-  for (long long blk = blockIdx.x; blk < nblk; blk += gridDim.x) {
-    long long r0, r1;
-    gn_det_block_range(blk, hw, r0, r1);
-    gn_det_block_partial(xs, r0, r1, ldx, C, groups, s_red, ps + blk * groups);
-  }
-  // grid-wide barrier (sense reversal, as in gn_fused_kernel)
+__device__ __forceinline__ void gn_grid_barrier(GnBarrier* bar) {
   __syncthreads();
   if (threadIdx.x == 0) {
     const unsigned int total = gridDim.x * gridDim.y;
@@ -567,23 +233,145 @@ gn_det_fused_kernel(const bf16* __restrict__ x, bf16* __restrict__ y, const floa
     }
   }
   __syncthreads();
-  float* s_stat = s_red;
-  gn_det_fold(ps, nblk, groups, static_cast<double>(rows_per_sample) * (C / groups), eps, s_stat);
+}
+
+// stats[sample][group] = {sum, sumsq} (double), accumulated with atomics: smem float atomics per channel, then fp64
+// global atomics per group.  grid = (row chunks of rows_per_cta, samples).
+__global__ void __launch_bounds__(512)
+gn_stats_kernel(const bf16* __restrict__ x, double* __restrict__ stats, long long rows_per_sample, int C,
+                long long ldx, int groups, int rows_per_cta) {
+  extern __shared__ float s_acc[];  // [2][C]
+  const int vpr = C >> 3;
+  const int sample = blockIdx.y;
+  const long long row0 = static_cast<long long>(blockIdx.x) * rows_per_cta;
+  long long row1 = row0 + rows_per_cta;
+  if (row1 > rows_per_sample) row1 = rows_per_sample;
+  for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) s_acc[i] = 0.f;
   __syncthreads();
-  float sc[8], sh[8];
-  gn_det_scale_shift(s_stat, gamma, beta, C, groups, sc, sh);
-  const int vc = threadIdx.x % (C >> 3);
-  const bf16* xb = xs + vc * 8;
-  bf16* yb = y + static_cast<long long>(sample) * rows_per_sample * C + vc * 8;
-  if (static_cast<long long>(blockIdx.x) >= nblk) return;
-  const long long last = blockIdx.x + (nblk - 1 - blockIdx.x) / gridDim.x * gridDim.x;
-  for (long long blk = last; blk >= 0; blk -= gridDim.x) {
-    long long r0, r1;
-    gn_det_block_range(blk, hw, r0, r1);
-    gn_det_apply_rows(xb, yb, r0, r1, ldx, C, sc, sh, silu);
+  const int lanes_r = blockDim.x / vpr;
+  const int vc = threadIdx.x % vpr;
+  const int rl = threadIdx.x / vpr;
+  float s[8], q[8];
+  gn_col_sums(x + (static_cast<long long>(sample) * rows_per_sample) * ldx + vc * 8, row0, row1, ldx, lanes_r, rl, s, q);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    atomicAdd(&s_acc[vc * 8 + j], s[j]);
+    atomicAdd(&s_acc[C + vc * 8 + j], q[j]);
+  }
+  __syncthreads();
+  const int cg = C / groups;
+  for (int g = threadIdx.x; g < groups; g += blockDim.x) {
+    double ds = 0.0, dq = 0.0;
+    for (int c = 0; c < cg; ++c) {
+      ds += static_cast<double>(s_acc[g * cg + c]);
+      dq += static_cast<double>(s_acc[C + g * cg + c]);
+    }
+    double* o = stats + (static_cast<long long>(sample) * groups + g) * 2;
+    atomicAdd(o, ds);
+    atomicAdd(o + 1, dq);
   }
 }
 
+// The block pairs of the deterministic statistics: grid = (blocks per sample, samples), one CTA per block;
+// partial = float2 [samples][ldp][groups].
+__global__ void __launch_bounds__(512)
+gn_partials_kernel(const bf16* __restrict__ x, float2* __restrict__ partial, long long rows_per_sample, long long hw,
+                   int C, long long ldx, int groups, long long ldp) {
+  extern __shared__ float s_red[];  // [2][lanes_r][C]
+  const int vpr = C >> 3;
+  const int sample = blockIdx.y;
+  long long r0, r1;
+  gn_block_range(blockIdx.x, hw, gn_det_block_rows(hw), r0, r1);
+  float s[8], q[8];
+  gn_col_sums(x + static_cast<long long>(sample) * rows_per_sample * ldx + (threadIdx.x % vpr) * 8, r0, r1, ldx,
+              blockDim.x / vpr, threadIdx.x / vpr, s, q);
+  gn_cta_pairs(s, q, C, groups, s_red, partial + (static_cast<long long>(sample) * ldp + blockIdx.x) * groups);
+}
+
+// Where the apply kernel's mean / rstd come from: fp64 (sum, sumsq) [samples][groups][2] of gn_stats_kernel ...
+struct GnStatsF64 {
+  const double* stats;
+  __device__ __forceinline__ void operator()(int sample, int groups, double cnt, float eps, float* s_stat) const {
+    const double* st = stats + static_cast<long long>(sample) * groups * 2;
+    for (int g = threadIdx.x; g < groups; g += blockDim.x) gn_set_stat(s_stat, g, st[2 * g], st[2 * g + 1], cnt, eps);
+  }
+};
+// ... or the fold of nblk block pairs per sample ([samples][nblk][groups])
+struct GnFoldPartials {
+  const float2* partial;
+  long long nblk;
+  __device__ __forceinline__ void operator()(int sample, int groups, double cnt, float eps, float* s_stat) const {
+    gn_fold(partial + static_cast<long long>(sample) * nblk * groups, nblk, groups, cnt, eps, s_stat);
+  }
+};
+
+// grid = (row chunks of rows_per_cta, samples): mean / rstd of the sample's groups over count_rows x C/groups
+// elements, then normalise the CTA's rows.
+template <class Stat>
+__global__ void __launch_bounds__(512)
+gn_apply_kernel(const bf16* __restrict__ x, bf16* __restrict__ y, Stat stat, const float* __restrict__ gamma,
+                const float* __restrict__ beta, long long rows_per_sample, long long count_rows, int C, long long ldx,
+                int groups, float eps, int silu, int rows_per_cta) {
+  extern __shared__ float s_stat[];  // [groups][2]
+  const int vpr = C >> 3;
+  const int vc = threadIdx.x % vpr;
+  const int sample = blockIdx.y;
+  stat(sample, groups, static_cast<double>(count_rows) * (C / groups), eps, s_stat);
+  __syncthreads();
+  float sc[8], sh[8];
+  gn_scale_shift(s_stat, gamma, beta, C, groups, sc, sh);
+  const long long row0 = static_cast<long long>(blockIdx.x) * rows_per_cta;
+  const long long row1 = row0 + rows_per_cta < rows_per_sample ? row0 + rows_per_cta : rows_per_sample;
+  const long long srow = static_cast<long long>(sample) * rows_per_sample;
+  gn_apply_rows<false>(x + srow * ldx + vc * 8, y + srow * static_cast<long long>(C) + vc * 8, row0, row1, ldx, C,
+                       blockDim.x / vpr, threadIdx.x / vpr, sc, sh, silu);
+}
+
+// GroupNorm in ONE launch: the CTAs of a sample stride over its blocks (CTA i takes blocks i, i + gridDim.x, ...) and
+// write the block pairs, a grid barrier (the grid is sized to be co-resident), then EVERY CTA folds all blocks of its
+// sample (so the fold does not depend on gridDim) and normalises the rows of its own blocks, last row first (the rows
+// read last are the ones most likely still in the 50 MB L2).  One launch and one HBM read less than a two-kernel pair.
+// MAXT / MINB: launch bounds.  <256, 3> (80 registers) is what every width up to C = 2048 uses: three 240-256-thread
+// CTAs per SM instead of two keep enough loads in flight for the streaming phases; wider rows take <512, 1>.
+// ONE: one block per CTA (the default mode: hw = rows_per_sample, gridDim.x blocks), which drops the block loops and
+// their 64-bit divisions from the short per-CTA prologue / epilogue.
+template <int MAXT, int MINB, bool ONE>
+__global__ void __launch_bounds__(MAXT, MINB)
+gn_fused_kernel(const bf16* __restrict__ x, bf16* __restrict__ y, const float* __restrict__ gamma,
+                const float* __restrict__ beta, GnBarrier* __restrict__ bar, float2* __restrict__ partial,
+                long long rows_per_sample, long long hw, long long R, int C, long long ldx, int groups, float eps,
+                int silu) {
+  extern __shared__ float s_red[];  // [2][lanes_r][C] thread sums, reused as s_stat [groups][2]
+  const int vpr = C >> 3;
+  const int lanes_r = blockDim.x / vpr;
+  const int vc = threadIdx.x % vpr;
+  const int rl = threadIdx.x / vpr;
+  const int sample = blockIdx.y;
+  const long long nblk = ONE ? gridDim.x : rows_per_sample / hw * gn_blocks_per_frame(hw, R);
+  const long long srow = static_cast<long long>(sample) * rows_per_sample;
+  const bf16* xb = x + srow * ldx + vc * 8;
+  float2* ps = partial + static_cast<long long>(sample) * nblk * groups;
+  for (long long blk = blockIdx.x; blk < nblk; blk += gridDim.x) {
+    long long r0, r1;
+    gn_block_range<ONE>(blk, hw, R, r0, r1);
+    float s[8], q[8];
+    gn_col_sums(xb, r0, r1, ldx, lanes_r, rl, s, q);
+    gn_cta_pairs(s, q, C, groups, s_red, ps + blk * groups);
+  }
+  gn_grid_barrier(bar);
+  gn_fold(ps, nblk, groups, static_cast<double>(rows_per_sample) * (C / groups), eps, s_red);
+  __syncthreads();
+  float sc[8], sh[8];
+  gn_scale_shift(s_red, gamma, beta, C, groups, sc, sh);
+  if (static_cast<long long>(blockIdx.x) >= nblk) return;
+  bf16* yb = y + srow * static_cast<long long>(C) + vc * 8;
+  const long long last = ONE ? blockIdx.x : blockIdx.x + (nblk - 1 - blockIdx.x) / gridDim.x * gridDim.x;
+  for (long long blk = last; blk >= 0; blk -= gridDim.x) {
+    long long r0, r1;
+    gn_block_range<ONE>(blk, hw, R, r0, r1);
+    gn_apply_rows<true>(xb, yb, r0, r1, ldx, C, lanes_r, rl, sc, sh, silu);
+  }
+}
 // ------------------------------------------------------------------------------------------------
 // LayerNorm over C (<= 2048), one warp per row, row held in registers.
 //   z = x[row] + add[row / rows_per_frame]   (add optional, fp32)
@@ -891,6 +679,87 @@ static int pick_rows_per_cta(long long rows_per_sample, int nsamples) {
   return static_cast<int>(rpc);
 }
 
+// Launch shape of the GroupNorm kernels at width C: C / 8 vector columns x lanes_r row lanes (about kGnThreads
+// threads), and the [2][lanes_r][C] floats of the CTA tree (gn_cta_pairs).
+struct GnShape {
+  int lanes_r, threads;
+  size_t smem;
+};
+static GnShape gn_shape(int C) {
+  const int vpr = C / 8;
+  const int lanes_r = kGnThreads / vpr > 0 ? kGnThreads / vpr : 1;
+  return {lanes_r, vpr * lanes_r, sizeof(float) * 2 * static_cast<size_t>(lanes_r) * C};
+}
+
+// What every GroupNorm entry point requires of the shape
+static bool gn_shape_ok(int C, int ldx, int groups, long long rows_per_sample, int nsamples) {
+  return C > 0 && C % 8 == 0 && groups > 0 && C % groups == 0 && C / 8 <= 512 && ldx % 8 == 0 &&
+         rows_per_sample > 0 && nsamples > 0;
+}
+
+// Workspace of the single launch: the barrier words, then the block pairs (float2 [samples][blocks][groups]).
+constexpr size_t kGnWsHeader = 256;
+constexpr int kGnMaxCtas = 4096;  // CTAs the default mode's fixed-size workspace has pairs for
+static int64_t gn_ws_bytes(long long pairs) { return static_cast<int64_t>(kGnWsHeader + sizeof(float2) * pairs); }
+
+// gn_fused_kernel over nsamples x (CTAs per sample).  det: the blocks of min(256, hw) rows, which the CTAs of a
+// sample stride over; otherwise one block per CTA.  The grid barrier needs every CTA resident at once, so the grid is
+// held to the co-resident capacity (occupancy x SMs, at most 4 CTAs per SM and kGnMaxCtas in all);
+// V3D_ERR_UNSUPPORTED when nsamples exceeds it (the caller then takes the two-kernel form).
+static int gn_fused(const char* who, bool det, const void* x, void* y, const void* gamma, const void* beta,
+                    long long rows_per_sample, long long hw, int nsamples, int C, int ldx, int groups, float eps,
+                    int silu, void* workspace, void* stream) {
+  const GnShape sh = gn_shape(C);
+  auto kern = sh.threads <= 256 ? (det ? gn_fused_kernel<256, 3, false> : gn_fused_kernel<256, 3, true>)
+                                 : (det ? gn_fused_kernel<512, 1, false> : gn_fused_kernel<512, 1, true>);
+  int per_sm = 0;
+  const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, sh.threads, sh.smem);
+  if (e != cudaSuccess || per_sm < 1) {
+    set_error("%s: occupancy query failed (%s)", who, cudaGetErrorString(e));
+    return V3D_ERR_CUDA;
+  }
+  long long cap = static_cast<long long>(per_sm < 4 ? per_sm : 4) * num_sms();
+  if (cap > kGnMaxCtas) cap = kGnMaxCtas;
+  if (nsamples > cap) {
+    set_error("%s: %d samples exceed the co-resident grid (%lld CTAs)", who, nsamples, cap);
+    return V3D_ERR_UNSUPPORTED;
+  }
+  long long ctas = cap / nsamples, R;
+  if (det) {
+    R = gn_det_block_rows(hw);
+    const long long nblk = rows_per_sample / hw * gn_blocks_per_frame(hw, R);
+    if (ctas > nblk) ctas = nblk;
+  } else {
+    // >= 16 rows per thread: the barrier and the pairs must stay small next to the streaming loops
+    long long max_ctas = rows_per_sample / (16LL * sh.lanes_r);
+    if (max_ctas < 1) max_ctas = 1;
+    if (ctas > max_ctas) ctas = max_ctas;
+    hw = rows_per_sample;
+    R = (rows_per_sample + ctas - 1) / ctas;
+    ctas = (rows_per_sample + R - 1) / R;
+  }
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  kern<<<dim3(static_cast<unsigned>(ctas), nsamples), sh.threads, sh.smem, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const bf16*>(x), static_cast<bf16*>(y), static_cast<const float*>(gamma),
+      static_cast<const float*>(beta), reinterpret_cast<GnBarrier*>(ws), reinterpret_cast<float2*>(ws + kGnWsHeader),
+      rows_per_sample, hw, R, C, ldx, groups, eps, silu);
+  V3D_CHECK_LAUNCH("gn_fused_kernel");
+  return V3D_OK;
+}
+
+// gn_apply_kernel over row chunks of pick_rows_per_cta rows x nsamples
+template <class Stat>
+static int gn_apply(Stat stat, const void* x, void* y, const void* gamma, const void* beta, long long rows_per_sample,
+                    long long count_rows, int nsamples, int C, int ldx, int groups, float eps, int silu, void* stream) {
+  const int rpc = pick_rows_per_cta(rows_per_sample, nsamples);
+  gn_apply_kernel<<<dim3(static_cast<unsigned>((rows_per_sample + rpc - 1) / rpc), nsamples), gn_shape(C).threads,
+                    sizeof(float) * 2 * groups, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const bf16*>(x), static_cast<bf16*>(y), stat, static_cast<const float*>(gamma),
+      static_cast<const float*>(beta), rows_per_sample, count_rows, C, ldx, groups, eps, silu, rpc);
+  V3D_CHECK_LAUNCH("gn_apply_kernel");
+  return V3D_OK;
+}
+
 }  // namespace v3d
 
 using namespace v3d;
@@ -903,8 +772,7 @@ extern "C" {
  * time_stack ResBlock (openaimodel.py:267-271 with dims=3: reduction over (C/32, T, H, W)). */
 int v3d_groupnorm_stats(const void* x, void* stats, int64_t rows_per_sample, int32_t nsamples, int32_t C,
                         int32_t ldx, int32_t groups, int32_t pre_zeroed, void* stream) {
-  if (!x || !stats || C % 8 != 0 || C % groups != 0 || C / 8 > 512 || ldx % 8 != 0 ||
-      rows_per_sample <= 0 || nsamples <= 0) {
+  if (!x || !stats || !gn_shape_ok(C, ldx, groups, rows_per_sample, nsamples)) {
     set_error("v3d_groupnorm_stats: bad args C=%d groups=%d ldx=%d", C, groups, ldx);
     return V3D_ERR_BAD_ARG;
   }
@@ -917,11 +785,9 @@ int v3d_groupnorm_stats(const void* x, void* stats, int64_t rows_per_sample, int
     }
   }
   const int rpc = pick_rows_per_cta(rows_per_sample, nsamples);
-  dim3 grid(static_cast<unsigned>((rows_per_sample + rpc - 1) / rpc), nsamples);
-  const int vpr = C / 8;
-  const int lanes_r = kGnThreads / vpr > 0 ? kGnThreads / vpr : 1;
-  gn_stats_kernel<<<grid, vpr * lanes_r, 2 * C * sizeof(float), st>>>(
-      static_cast<const bf16*>(x), static_cast<double*>(stats), rows_per_sample, C, ldx, groups, rpc);
+  gn_stats_kernel<<<dim3(static_cast<unsigned>((rows_per_sample + rpc - 1) / rpc), nsamples), gn_shape(C).threads,
+                    2 * C * sizeof(float), st>>>(static_cast<const bf16*>(x), static_cast<double*>(stats),
+                                                 rows_per_sample, C, ldx, groups, rpc);
   V3D_CHECK_LAUNCH("gn_stats_kernel");
   return V3D_OK;
 }
@@ -931,30 +797,17 @@ int v3d_groupnorm_stats(const void* x, void* stats, int64_t rows_per_sample, int
 int v3d_groupnorm_apply(const void* x, void* y, const void* stats, const void* gamma, const void* beta,
                         int64_t rows_per_sample, int32_t nsamples, int32_t C, int32_t ldx, int32_t groups,
                         float eps, int32_t silu, void* stream) {
-  if (!x || !y || !stats || !gamma || !beta || C % 8 != 0 || C % groups != 0 || ldx % 8 != 0) {
-    set_error("v3d_groupnorm_apply: bad args");
+  if (!x || !y || !stats || !gamma || !beta || !gn_shape_ok(C, ldx, groups, rows_per_sample, nsamples)) {
+    set_error("v3d_groupnorm_apply: bad args C=%d groups=%d ldx=%d", C, groups, ldx);
     return V3D_ERR_BAD_ARG;
   }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (C / 8 > 512) {
-    set_error("v3d_groupnorm_apply: C=%d too wide", C);
-    return V3D_ERR_BAD_ARG;
-  }
-  const int rpc = pick_rows_per_cta(rows_per_sample, nsamples);
-  dim3 grid(static_cast<unsigned>((rows_per_sample + rpc - 1) / rpc), nsamples);
-  const int vpr = C / 8;
-  const int lanes_r = kGnThreads / vpr > 0 ? kGnThreads / vpr : 1;
-  gn_apply_kernel<<<grid, vpr * lanes_r, 0, st>>>(
-      static_cast<const bf16*>(x), static_cast<bf16*>(y), static_cast<const double*>(stats),
-      static_cast<const float*>(gamma), static_cast<const float*>(beta), rows_per_sample, C, ldx, groups,
-      eps, silu, rpc);
-  V3D_CHECK_LAUNCH("gn_apply_kernel");
-  return V3D_OK;
+  return gn_apply(GnStatsF64{static_cast<const double*>(stats)}, x, y, gamma, beta, rows_per_sample, rows_per_sample,
+                  nsamples, C, ldx, groups, eps, silu, stream);
 }
 
 /* Bytes of the workspace v3d_groupnorm needs (barrier words + per-CTA partials); the caller allocates it once per
  * stream, ZEROED, and passes the same buffer to every call on that stream. */
-int64_t v3d_groupnorm_workspace_bytes(void) { return static_cast<int64_t>(kGnWsBytes); }
+int64_t v3d_groupnorm_workspace_bytes(void) { return gn_ws_bytes(32LL * kGnMaxCtas); }
 
 /* y[dense, ld=C] = act(GroupNorm(x; gamma, beta, eps)) in ONE launch (statistics + grid barrier + apply); same
  * operand meaning as the v3d_groupnorm_stats / v3d_groupnorm_apply pair it replaces on the unsharded path
@@ -963,69 +816,28 @@ int64_t v3d_groupnorm_workspace_bytes(void) { return static_cast<int64_t>(kGnWsB
 int v3d_groupnorm(const void* x, void* y, const void* gamma, const void* beta, int64_t rows_per_sample,
                   int32_t nsamples, int32_t C, int32_t ldx, int32_t groups, float eps, int32_t silu,
                   void* workspace, int64_t workspace_bytes, void* stream) {
-  if (!x || !y || !gamma || !beta || !workspace || C % 8 != 0 || groups <= 0 || groups > 32 || C % groups != 0 ||
-      C / 8 > 512 || ldx % 8 != 0 || rows_per_sample <= 0 || nsamples <= 0 ||
-      workspace_bytes < static_cast<int64_t>(kGnWsBytes)) {
+  if (!x || !y || !gamma || !beta || !workspace || !gn_shape_ok(C, ldx, groups, rows_per_sample, nsamples) ||
+      groups > 32 || workspace_bytes < v3d_groupnorm_workspace_bytes()) {
     set_error("v3d_groupnorm: bad args C=%d groups=%d ldx=%d workspace=%lld", C, groups, ldx,
               static_cast<long long>(workspace_bytes));
     return V3D_ERR_BAD_ARG;
   }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int vpr = C / 8;
-  const int lanes_r = kGnThreads / vpr > 0 ? kGnThreads / vpr : 1;
-  const int threads = vpr * lanes_r;
-  const size_t smem = sizeof(float) * 2 * static_cast<size_t>(lanes_r) * C;
-  // co-resident capacity of this launch shape (the barrier needs every CTA on the device at once)
-  int per_sm = 0;
-  auto kern = threads <= 256 ? gn_fused_kernel<256, 3> : gn_fused_kernel<512, 1>;
-  cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem);
-  if (e != cudaSuccess || per_sm < 1) {
-    set_error("v3d_groupnorm: occupancy query failed (%s)", cudaGetErrorString(e));
-    return V3D_ERR_CUDA;
-  }
-  if (per_sm > 4) per_sm = 4;
-  long long cap = static_cast<long long>(per_sm) * num_sms();
-  if (cap > kGnMaxCtas) cap = kGnMaxCtas;
-  if (nsamples > cap) {
-    // more samples than co-resident CTAs: fall back to the two-kernel form on the caller's side
-    set_error("v3d_groupnorm: %d samples exceed the co-resident grid (%lld CTAs)", nsamples, cap);
-    return V3D_ERR_UNSUPPORTED;
-  }
-  long long chunks = cap / nsamples;
-  long long max_chunks = rows_per_sample / (16LL * lanes_r);  // >= 16 rows per thread: the barrier and the partials
-                                                              // must stay small next to the streaming loops
-  if (max_chunks < 1) max_chunks = 1;
-  if (chunks > max_chunks) chunks = max_chunks;
-  long long rpc = (rows_per_sample + chunks - 1) / chunks;
-  chunks = (rows_per_sample + rpc - 1) / rpc;
-  dim3 grid(static_cast<unsigned>(chunks), nsamples);
-  uint8_t* ws = static_cast<uint8_t*>(workspace);
-  kern<<<grid, threads, smem, st>>>(
-      static_cast<const bf16*>(x), static_cast<bf16*>(y), static_cast<const float*>(gamma),
-      static_cast<const float*>(beta), reinterpret_cast<GnBarrier*>(ws), reinterpret_cast<float2*>(ws + 256),
-      rows_per_sample, C, ldx, groups, eps, silu, static_cast<int>(rpc));
-  V3D_CHECK_LAUNCH("gn_fused_kernel");
-  return V3D_OK;
+  return gn_fused("v3d_groupnorm", false, x, y, gamma, beta, rows_per_sample, rows_per_sample, nsamples, C, ldx,
+                  groups, eps, silu, workspace, stream);
 }
 
 /* Deterministic GroupNorm: blocks per sample of the statistics definition (rows_per_sample = frames x hw, blocks of
  * min(256, hw) rows that never straddle a frame); -1 if hw does not divide rows_per_sample. */
 int64_t v3d_groupnorm_det_blocks(int64_t rows_per_sample, int64_t hw) {
   if (hw <= 0 || rows_per_sample <= 0 || rows_per_sample % hw != 0) return -1;
-  return rows_per_sample / hw * gn_det_blocks_per_frame(hw);
+  return rows_per_sample / hw * gn_blocks_per_frame(hw, gn_det_block_rows(hw));
 }
 
 /* Bytes of the workspace v3d_groupnorm_det needs for this shape (barrier words + one fp32 pair per block and group). */
 int64_t v3d_groupnorm_det_workspace_bytes(int64_t rows_per_sample, int64_t hw, int32_t nsamples, int32_t groups) {
   const int64_t nblk = v3d_groupnorm_det_blocks(rows_per_sample, hw);
   if (nblk < 0 || nsamples <= 0 || groups <= 0) return -1;
-  return 256 + static_cast<int64_t>(sizeof(float2)) * nblk * nsamples * groups;
-}
-
-static bool gn_det_args_ok(const void* x, int64_t rows_per_sample, int64_t hw, int32_t nsamples, int32_t C, int32_t ldx,
-                           int32_t groups) {
-  return x && C % 8 == 0 && groups > 0 && groups <= 32 && C % groups == 0 && C / 8 <= 512 && ldx % 8 == 0 &&
-         nsamples > 0 && v3d_groupnorm_det_blocks(rows_per_sample, hw) > 0;
+  return gn_ws_bytes(nblk * nsamples * groups);
 }
 
 /* Block partials of the deterministic statistics: partials = float2 [nsamples][ldp][groups], block k of sample s at
@@ -1033,18 +845,17 @@ static bool gn_det_args_ok(const void* x, int64_t rows_per_sample, int64_t hw, i
 int v3d_groupnorm_partials(const void* x, void* partials, int64_t rows_per_sample, int64_t hw, int32_t nsamples,
                            int32_t C, int32_t ldx, int32_t groups, int64_t ldp, void* stream) {
   const int64_t nblk = v3d_groupnorm_det_blocks(rows_per_sample, hw);
-  if (!gn_det_args_ok(x, rows_per_sample, hw, nsamples, C, ldx, groups) || !partials || ldp < nblk ||
-      nsamples > 65535) {
+  if (!x || !partials || !gn_shape_ok(C, ldx, groups, rows_per_sample, nsamples) || groups > 32 || nblk <= 0 ||
+      ldp < nblk || nsamples > 65535) {
     set_error("v3d_groupnorm_partials: bad args C=%d groups=%d ldx=%d hw=%lld ldp=%lld", C, groups, ldx,
               static_cast<long long>(hw), static_cast<long long>(ldp));
     return V3D_ERR_BAD_ARG;
   }
-  const int vpr = C / 8;
-  const int lanes_r = kGnThreads / vpr > 0 ? kGnThreads / vpr : 1;
-  gn_det_partials_kernel<<<dim3(static_cast<unsigned>(nblk), nsamples), vpr * lanes_r,
-                           sizeof(float) * 2 * static_cast<size_t>(lanes_r) * C, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const bf16*>(x), static_cast<float2*>(partials), rows_per_sample, hw, C, ldx, groups, ldp);
-  V3D_CHECK_LAUNCH("gn_det_partials_kernel");
+  const GnShape sh = gn_shape(C);
+  gn_partials_kernel<<<dim3(static_cast<unsigned>(nblk), nsamples), sh.threads, sh.smem,
+                       static_cast<cudaStream_t>(stream)>>>(static_cast<const bf16*>(x), static_cast<float2*>(partials),
+                                                            rows_per_sample, hw, C, ldx, groups, ldp);
+  V3D_CHECK_LAUNCH("gn_partials_kernel");
   return V3D_OK;
 }
 
@@ -1054,22 +865,14 @@ int v3d_groupnorm_partials(const void* x, void* partials, int64_t rows_per_sampl
 int v3d_groupnorm_fold_apply(const void* x, void* y, const void* partials, const void* gamma, const void* beta,
                              int64_t rows_per_sample, int32_t nsamples, int32_t C, int32_t ldx, int32_t groups,
                              int64_t nblocks, int64_t count_rows, float eps, int32_t silu, void* stream) {
-  if (!gn_det_args_ok(x, rows_per_sample, rows_per_sample, nsamples, C, ldx, groups) || !y || !partials || !gamma ||
-      !beta || nblocks <= 0 || count_rows <= 0 || nsamples > 65535) {
+  if (!x || !y || !partials || !gamma || !beta || !gn_shape_ok(C, ldx, groups, rows_per_sample, nsamples) ||
+      groups > 32 || nblocks <= 0 || count_rows <= 0 || nsamples > 65535) {
     set_error("v3d_groupnorm_fold_apply: bad args C=%d groups=%d ldx=%d nblocks=%lld", C, groups, ldx,
               static_cast<long long>(nblocks));
     return V3D_ERR_BAD_ARG;
   }
-  const int rpc = pick_rows_per_cta(rows_per_sample, nsamples);
-  const int vpr = C / 8;
-  const int lanes_r = kGnThreads / vpr > 0 ? kGnThreads / vpr : 1;
-  gn_det_apply_kernel<<<dim3(static_cast<unsigned>((rows_per_sample + rpc - 1) / rpc), nsamples), vpr * lanes_r, 0,
-                        static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const bf16*>(x), static_cast<bf16*>(y), static_cast<const float2*>(partials),
-      static_cast<const float*>(gamma), static_cast<const float*>(beta), rows_per_sample, C, ldx, groups, nblocks,
-      count_rows, eps, silu, rpc);
-  V3D_CHECK_LAUNCH("gn_det_apply_kernel");
-  return V3D_OK;
+  return gn_apply(GnFoldPartials{static_cast<const float2*>(partials), nblocks}, x, y, gamma, beta, rows_per_sample,
+                  count_rows, nsamples, C, ldx, groups, eps, silu, stream);
 }
 
 /* The deterministic normalisation in ONE launch; bit-identical to v3d_groupnorm_partials + v3d_groupnorm_fold_apply.
@@ -1079,41 +882,14 @@ int v3d_groupnorm_det(const void* x, void* y, const void* gamma, const void* bet
                       int32_t nsamples, int32_t C, int32_t ldx, int32_t groups, float eps, int32_t silu,
                       void* workspace, int64_t workspace_bytes, void* stream) {
   const int64_t need = v3d_groupnorm_det_workspace_bytes(rows_per_sample, hw, nsamples, groups);
-  if (!gn_det_args_ok(x, rows_per_sample, hw, nsamples, C, ldx, groups) || !y || !gamma || !beta || !workspace ||
-      workspace_bytes < need) {
+  if (!x || !y || !gamma || !beta || !workspace || !gn_shape_ok(C, ldx, groups, rows_per_sample, nsamples) ||
+      groups > 32 || need < 0 || workspace_bytes < need) {
     set_error("v3d_groupnorm_det: bad args C=%d groups=%d ldx=%d hw=%lld workspace=%lld (need %lld)", C, groups, ldx,
               static_cast<long long>(hw), static_cast<long long>(workspace_bytes), static_cast<long long>(need));
     return V3D_ERR_BAD_ARG;
   }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int vpr = C / 8;
-  const int lanes_r = kGnThreads / vpr > 0 ? kGnThreads / vpr : 1;
-  const int threads = vpr * lanes_r;
-  size_t smem = sizeof(float) * 2 * static_cast<size_t>(lanes_r) * C;
-  if (smem < sizeof(float) * 2 * groups) smem = sizeof(float) * 2 * groups;
-  int per_sm = 0;
-  auto kern = threads <= 256 ? gn_det_fused_kernel<256, 3> : gn_det_fused_kernel<512, 1>;
-  cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem);
-  if (e != cudaSuccess || per_sm < 1) {
-    set_error("v3d_groupnorm_det: occupancy query failed (%s)", cudaGetErrorString(e));
-    return V3D_ERR_CUDA;
-  }
-  if (per_sm > 4) per_sm = 4;
-  const long long cap = static_cast<long long>(per_sm) * num_sms();
-  if (nsamples > cap) {
-    set_error("v3d_groupnorm_det: %d samples exceed the co-resident grid (%lld CTAs)", nsamples, cap);
-    return V3D_ERR_UNSUPPORTED;
-  }
-  long long chunks = cap / nsamples;
-  const long long nblk = v3d_groupnorm_det_blocks(rows_per_sample, hw);
-  if (chunks > nblk) chunks = nblk;
-  uint8_t* ws = static_cast<uint8_t*>(workspace);
-  kern<<<dim3(static_cast<unsigned>(chunks), nsamples), threads, smem, st>>>(
-      static_cast<const bf16*>(x), static_cast<bf16*>(y), static_cast<const float*>(gamma),
-      static_cast<const float*>(beta), reinterpret_cast<GnBarrier*>(ws), reinterpret_cast<float2*>(ws + 256),
-      rows_per_sample, hw, C, ldx, groups, eps, silu);
-  V3D_CHECK_LAUNCH("gn_det_fused_kernel");
-  return V3D_OK;
+  return gn_fused("v3d_groupnorm_det", true, x, y, gamma, beta, rows_per_sample, hw, nsamples, C, ldx, groups, eps,
+                  silu, workspace, stream);
 }
 
 /* LayerNorm (attention.py:525-527, video_attention.py:51,79,93-94) with the optional fused

@@ -193,6 +193,13 @@ int v3d_attention_temporal(const void* q, const void* k, const void* v, void* o,
 int v3d_attention_temporal_kv(const void* q, const void* k, const void* v, void* o, int64_t ld_q, int64_t ld_kv,
                               int64_t ld_o, int32_t nb, int32_t Tq, int32_t Tk, int32_t S, int32_t nheads,
                               const int32_t* kv_row, const int32_t* kv_bstride, float scale, void* stream);
+/* CrossAttention over a context of nk >= 1 tokens (attention.py:286-349; the spatial and temporal attn2 of a
+ * multi-token context), on the wgmma kernel of v3d_attention_spatial: item b's nq query rows b*nq + i (row stride ld_q)
+ * attend to its own key / value rows b*kv_bstride + j, j < nk (row stride ld_kv, kv_bstride >= nk; rows between key
+ * sets are not read); output rows b*nq + i, row stride ld_o. */
+int v3d_attention_cross(const void* q, const void* k, const void* v, void* o, int64_t ld_q, int64_t ld_kv,
+                        int64_t ld_o, int32_t nbatch, int32_t nq, int32_t nk, int64_t kv_bstride, int32_t nheads,
+                        float scale, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Data movement / small matrices (elementwise.cu)

@@ -8,6 +8,7 @@ exchange replaced by a byte counter.  Nothing is computed; this is bookkeeping o
     python tools/schedule_cost.py                      # V3D_512: one UNet forward (B=36) + one decode, per family
     python tools/schedule_cost.py --plan views --world 8 --rank 0      # this rank's share when frame-sharded
     python tools/schedule_cost.py --frames 24 --json out.json
+    python tools/schedule_cost.py --tokens 4                   # a 4-token cross-attention context (default 1)
 """
 from __future__ import annotations
 
@@ -103,6 +104,12 @@ def attention_temporal_kv(q, kv, out, nb, tq, s, nheads, kv_row, kv_bstride, sca
     return out
 
 
+def attention_cross(q, kv, out, nbatch, nq, nk, nheads, scale, kv_bstride=None):
+    # Q read and O written once per query row, the item's K / V once per (item, query tile) -- counted once here
+    book("attention_cross", 4.0 * nbatch * nq * nk * nheads * 64, (2 * nq + 2 * nk) * nbatch * nheads * 64 * 2)
+    return out
+
+
 def upsample_nearest2x(x, y, n, h, w, c):
     book("upsample_nearest2x", 0, 5 * n * h * w * c * 2)
     return y
@@ -143,7 +150,7 @@ def time_mix_conv(x, ldx, w, bias, y, nb, t, hw, c):
 
 
 COUNTERS = ["gemm", "groupnorm_stats", "groupnorm_apply", "groupnorm", "groupnorm_workspace", "layernorm", "softmax_rows_f32", "attention_spatial",
-            "attention_temporal", "attention_temporal_kv", "upsample_nearest2x", "copy_channels", "im2col3x3",
+            "attention_temporal", "attention_temporal_kv", "attention_cross", "upsample_nearest2x", "copy_channels", "im2col3x3",
             "nchw_f32_to_nhwc_bf16", "nhwc_to_nchw_f32", "small_linear", "timestep_embedding", "time_mix_conv"]
 
 
@@ -193,7 +200,7 @@ def _realise_mix_factors(mod: nn.Module) -> None:
             owner._parameters[name.split(".")[-1]] = nn.Parameter(torch.zeros(p.shape), requires_grad=False)
 
 
-def run(frames: int, latent: int, plan: str, world: int, rank: int, edm_steps: int):
+def run(frames: int, latent: int, plan: str, world: int, rank: int, edm_steps: int, tokens: int = 1):
     cfg = engine.v3d_512_config(num_frames=frames)
     with torch.device("meta"):
         eng = engine.DiffusionEngine(**cfg)
@@ -212,7 +219,7 @@ def run(frames: int, latent: int, plan: str, world: int, rank: int, edm_steps: i
     with counting(), torch.no_grad():
         Pu = unet._pack(META)
         x = torch.empty(B, 8, latent, latent, device=META)
-        ctx = torch.empty(B + (nb if vs is not None else 0), 1024, device=META)
+        ctx = torch.empty(B + (nb if vs is not None else 0), tokens * 1024, device=META)
         unet.view_shard = vs
         unet._run(Pu, x, torch.empty(B, device=META), ctx, torch.empty(B, 768, device=META), B, tl, nb, latent, latent,
                   META)
@@ -240,7 +247,7 @@ def run(frames: int, latent: int, plan: str, world: int, rank: int, edm_steps: i
         COMM.clear()
     cfg_bytes = tl * 4 * latent * latent * 4 if nb == 1 else 0      # one denoised half per network evaluation
     return {"config": {"frames": frames, "latent": latent, "plan": plan, "world": world, "rank": rank,
-                       "unet_batch": B, "frames_local": tl, "edm_steps": edm_steps},
+                       "unet_batch": B, "frames_local": tl, "edm_steps": edm_steps, "context_tokens": tokens},
             "unet_forward": unet_book, "decode": dec_book,
             "comm_per_unet_forward": dict(unet_comm, cfg_gather=[1 if nb == 1 else 0, cfg_bytes]),
             "comm_per_decode": dec_comm}
@@ -264,12 +271,13 @@ def main():
     ap.add_argument("--plan", choices=["none", "views", "cfg", "cfg+views"], default="none")
     ap.add_argument("--world", type=int, default=1)
     ap.add_argument("--rank", type=int, default=0)
+    ap.add_argument("--tokens", type=int, default=1, help="cross-attention context tokens per frame")
     ap.add_argument("--json", default=None)
     a = ap.parse_args()
-    res = run(a.frames, a.latent, a.plan, a.world, a.rank, a.edm_steps)
+    res = run(a.frames, a.latent, a.plan, a.world, a.rank, a.edm_steps, a.tokens)
     c = res["config"]
     print(f"schedule cost: T={c['frames']} latent {c['latent']}^2, plan {c['plan']} (world {c['world']}, rank {c['rank']}): "
-          f"UNet batch {c['unet_batch']}, {c['frames_local']} local frames")
+          f"UNet batch {c['unet_batch']}, {c['frames_local']} local frames, {c['context_tokens']} context token(s)")
     tu = table("one UNet forward", res["unet_forward"])
     td = table("one first-stage decode", res["decode"])
     S = a.edm_steps

@@ -80,6 +80,7 @@ SIGNATURES = {
     "v3d_attention_temporal": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _f32, _vp]),
     "v3d_attention_temporal_kv": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _i32, _i32, _i32,
                                             C.POINTER(C.c_int32), C.POINTER(C.c_int32), _f32, _vp]),
+    "v3d_attention_cross": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _i32, _i64, _i32, _f32, _vp]),
     # elementwise.cu
     "v3d_upsample_nearest2x": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp]),
     "v3d_copy_channels": (C.c_int, [_vp, _i64, _vp, _i64, _i64, _i32, _vp]),

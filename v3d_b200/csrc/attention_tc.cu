@@ -9,6 +9,10 @@
 //                                   bf16), B = V_j MN-major in shared memory
 // O and the running max / sum stay in registers for the whole key loop; when the row maximum grows, O and the sum are
 // rescaled in place.  Shared memory ~65 KB, so several CTAs share an SM and one CTA's softmax overlaps another's MMAs.
+//
+// The same kernel serves self-attention (nq = nk = the item's tokens, one tensor map shape for Q, K and V) and
+// cross-attention (nq queries of an item against its own nk keys, a separate K/V tensor map whose batch stride picks the
+// item's key set).  Keys past nk arrive zero-filled from TMA and are masked to -inf in the tail tile.
 #include <cstdlib>
 #include <type_traits>
 
@@ -57,7 +61,7 @@ __device__ __forceinline__ void exp2_poly2(float x0, float x1, float& p0, float&
 template <int POLY>
 __global__ void __launch_bounds__(AT_THREADS, 2)
 attn_tc_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-               const __grid_constant__ CUtensorMap mapV, bf16* __restrict__ O, long long ldo, int ntok,
+               const __grid_constant__ CUtensorMap mapV, bf16* __restrict__ O, long long ldo, int nq, int nk,
                float scale_log2e) {
   extern __shared__ uint8_t at_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(at_smem_raw) + 1023) &
@@ -71,7 +75,7 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__
   const int q0 = blockIdx.x * AT_BM;
   const int head = blockIdx.y;
   const int b = blockIdx.z;
-  const int nkv = (ntok + AT_BN - 1) / AT_BN;
+  const int nkv = (nk + AT_BN - 1) / AT_BN;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&mapQ);
@@ -135,7 +139,7 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__
       for (int c = 0; c < 8; ++c)
 #pragma unroll
         for (int e = 0; e < 2; ++e)
-          if (kbase + 8 * c + cq + e >= ntok) s[4 * c + e] = s[4 * c + 2 + e] = -INFINITY;
+          if (kbase + 8 * c + cq + e >= nk) s[4 * c + e] = s[4 * c + 2 + e] = -INFINITY;
     }
     float msc[2];
 #pragma unroll
@@ -145,7 +149,7 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__
       for (int c = 0; c < 8; ++c) mx = fmaxf(mx, fmaxf(s[4 * c + 2 * h], s[4 * c + 2 * h + 1]));
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-      // every key tile holds at least one key < ntok, so mx is finite
+      // every key tile holds at least one key < nk, so mx is finite
       if (mx > m_run[h]) {
         const float fac = ex2_approx((m_run[h] - mx) * scale_log2e);  // 0 on the first tile
         m_run[h] = mx;
@@ -170,8 +174,8 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__
         if (POLY != 0 && (POLY == 1 ? (c & 3) == 3 : (POLY == 2 ? (c & 1) == 1 : (c & 3) != 0))) {
           exp2_poly2(x0, x1, p0, p1);
           if (TAIL) {  // the polynomial clamps -inf to 2^-126
-            if (kbase + 8 * c + cq >= ntok) p0 = 0.f;
-            if (kbase + 8 * c + cq + 1 >= ntok) p1 = 0.f;
+            if (kbase + 8 * c + cq >= nk) p0 = 0.f;
+            if (kbase + 8 * c + cq + 1 >= nk) p1 = 0.f;
           }
         } else {
           p0 = ex2_approx(x0);
@@ -194,7 +198,7 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__
   uint32_t ph = 0;
   for (int j = 0; j < nkv; ++j) {
     mbar_wait(&kv_full[st], ph);
-    if (j * AT_BN + AT_BN > ntok) key_tile(j, st, std::true_type{});
+    if (j * AT_BN + AT_BN > nk) key_tile(j, st, std::true_type{});
     else key_tile(j, st, std::false_type{});
     if (wg_leader) mbar_arrive(&kv_empty[st]);
     if (++st == AT_KVSTAGES) {
@@ -211,8 +215,8 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     const float inv = 1.0f / l;
     const int row = q0 + cw * 64 + wi * 16 + (lane >> 2) + 8 * h;
-    if (row < ntok) {
-      bf16* op = O + (static_cast<long long>(b) * ntok + row) * ldo + head * 64 + cq;
+    if (row < nq) {
+      bf16* op = O + (static_cast<long long>(b) * nq + row) * ldo + head * 64 + cq;
 #pragma unroll
       for (int c = 0; c < 8; ++c)
         *reinterpret_cast<uint32_t*>(op + 8 * c) = pack_bf16x2(o[4 * c + 2 * h] * inv, o[4 * c + 2 * h + 1] * inv);
@@ -254,7 +258,7 @@ int v3d_attention_spatial(const void* q, const void* k, const void* v, void* o, 
     poly = v ? atoi(v) : 0;
     if (poly < 0 || poly > 3) poly = 0;
   }
-  using Kern = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, bf16*, long long, int, float);
+  using Kern = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, bf16*, long long, int, int, float);
   static const Kern kerns[4] = {attn_tc_kernel<0>, attn_tc_kernel<1>, attn_tc_kernel<2>, attn_tc_kernel<3>};
   static bool cfg[4] = {false, false, false, false};
   if (!cfg[poly]) {
@@ -267,7 +271,51 @@ int v3d_attention_spatial(const void* q, const void* k, const void* v, void* o, 
   }
   dim3 grid((ntok + AT_BM - 1) / AT_BM, nheads, nbatch);
   kerns[poly]<<<grid, AT_THREADS, AT_SMEM, static_cast<cudaStream_t>(stream)>>>(
-      mq, mk, mv, static_cast<bf16*>(o), ld_o, ntok, scale * 1.44269504088896340736f);
+      mq, mk, mv, static_cast<bf16*>(o), ld_o, ntok, ntok, scale * 1.44269504088896340736f);
+  V3D_CHECK_LAUNCH("attn_tc_kernel");
+  return V3D_OK;
+}
+
+/* softmax(q k^T * scale) v per (item, head), head dim 64, queries and keys from different matrices: item b's nq query
+ * rows (b*nq + i, row stride ld_q) attend to its own nk key / value rows b*kv_bstride + j (row stride ld_kv; k and v
+ * are column slices of one matrix), output rows b*nq + i (row stride ld_o).  kv_bstride >= nk; rows between key sets
+ * are never read.  Replaces CrossAttention.forward over a context of nk tokens, sgm/modules/attention.py:286-349:
+ * the spatial attn2 (each frame's own context, attention.py:571-572; kv_bstride = nk) and the temporal attn2 (the
+ * context of frame 0 of each video, time_context = context[::T], sgm/modules/video_attention.py:244-253,131;
+ * kv_bstride = T*nk read in place from the per-frame K/V rows). */
+int v3d_attention_cross(const void* q, const void* k, const void* v, void* o, int64_t ld_q, int64_t ld_kv,
+                        int64_t ld_o, int32_t nbatch, int32_t nq, int32_t nk, int64_t kv_bstride, int32_t nheads,
+                        float scale, void* stream) {
+  if (!q || !k || !v || !o || ld_q % 8 != 0 || ld_kv % 8 != 0 || ld_o % 8 != 0 || nbatch <= 0 || nq <= 0 || nk <= 0 ||
+      kv_bstride < nk || nheads <= 0 || nheads > 65535 || nbatch > 65535 || ld_q < nheads * 64LL ||
+      ld_kv < nheads * 64LL || ld_o < nheads * 64LL) {
+    set_error("v3d_attention_cross: bad args");
+    return V3D_ERR_BAD_ARG;
+  }
+  CUtensorMap mq, mk, mv;
+  const uint64_t dq[3] = {static_cast<uint64_t>(nheads) * 64, static_cast<uint64_t>(nq), static_cast<uint64_t>(nbatch)};
+  const uint64_t sq[2] = {static_cast<uint64_t>(ld_q) * 2, static_cast<uint64_t>(ld_q) * 2 * nq};
+  const uint64_t dkv[3] = {static_cast<uint64_t>(nheads) * 64, static_cast<uint64_t>(nk),
+                           static_cast<uint64_t>(nbatch)};
+  const uint64_t skv[2] = {static_cast<uint64_t>(ld_kv) * 2, static_cast<uint64_t>(ld_kv) * 2 * kv_bstride};
+  const uint32_t box_q[3] = {64, AT_BM, 1};
+  const uint32_t box_kv[3] = {64, AT_BN, 1};
+  int rc;
+  if ((rc = make_tmap_bf16(&mq, q, 3, dq, sq, box_q))) return rc;
+  if ((rc = make_tmap_bf16(&mk, k, 3, dkv, skv, box_kv))) return rc;
+  if ((rc = make_tmap_bf16(&mv, v, 3, dkv, skv, box_kv))) return rc;
+  static bool cfg = false;
+  if (!cfg) {
+    cudaError_t e = cudaFuncSetAttribute(attn_tc_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, AT_SMEM);
+    if (e != cudaSuccess) {
+      set_error("attn_tc smem attr: %s", cudaGetErrorString(e));
+      return V3D_ERR_CUDA;
+    }
+    cfg = true;
+  }
+  dim3 grid((nq + AT_BM - 1) / AT_BM, nheads, nbatch);
+  attn_tc_kernel<0><<<grid, AT_THREADS, AT_SMEM, static_cast<cudaStream_t>(stream)>>>(
+      mq, mk, mv, static_cast<bf16*>(o), ld_o, nq, nk, scale * 1.44269504088896340736f);
   V3D_CHECK_LAUNCH("attn_tc_kernel");
   return V3D_OK;
 }

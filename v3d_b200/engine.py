@@ -195,7 +195,7 @@ class DiffusionEngine(nn.Module):
         nb = 1 if cs is not None else 2
         extra = {"image_only_indicator": torch.zeros(nb, tl, device=randn.device), "num_video_frames": tl}
         if vs is not None:
-            tc = vs.time_context(c, uc)                       # [2, 1, ctx] in [uc; c] order
+            tc = vs.time_context(c, uc)                       # [2, M, ctx] in [uc; c] order
             extra["time_context"] = tc[cs.rank:cs.rank + 1] if cs is not None else tc
 
         def denoiser(inp, sigma, cond):

@@ -309,6 +309,23 @@ def attention_temporal_kv(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, 
     return out
 
 
+def attention_cross(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, nbatch: int, nq: int, nk: int, nheads: int,
+                    scale: float, kv_bstride: Optional[int] = None) -> torch.Tensor:
+    """Cross-attention over nk context tokens: q = [nbatch*nq, >= C] query rows (a column slice of a wider matrix is
+    fine: the row stride is taken from the tensor), kv = K | V in columns [0, C) and [C, 2C) of a row-strided view,
+    item b's keys at rows b*kv_bstride + j (default kv_bstride = nk), out = [nbatch*nq, >= C]."""
+    _need(q, torch.bfloat16, "attention q")
+    _need(kv, torch.bfloat16, "attention kv")
+    _need(out, torch.bfloat16, "attention out")
+    c = nheads * 64
+    base = kv.data_ptr()
+    _lib.check(_lib.load().v3d_attention_cross(q.data_ptr(), base, base + c * kv.element_size(), out.data_ptr(),
+                                               q.stride(0), kv.stride(0), out.stride(0), nbatch, nq, nk,
+                                               nk if kv_bstride is None else kv_bstride, nheads, scale, _stream()),
+               "v3d_attention_cross")
+    return out
+
+
 def upsample_nearest2x(x: torch.Tensor, y: torch.Tensor, n: int, h: int, w: int, c: int) -> torch.Tensor:
     _lib.check(_lib.load().v3d_upsample_nearest2x(x.data_ptr(), y.data_ptr(), n, h, w, c, _stream()),
                "v3d_upsample_nearest2x")

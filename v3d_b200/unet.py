@@ -651,8 +651,8 @@ class VideoUNet(KernelModule):
                     dense(base + ".ff.net.2")
                     for n_ in norms:
                         affine(f"{base}.{n_}")
-                    # single-token cross-attention collapses to to_out(to_v(ctx)) (SURVEY.md §0.4);
-                    # norm2 / to_q / to_k of attn2 cannot influence the result and are not packed.
+                    # single-token cross-attention collapses to to_out(to_v(ctx)) (SURVEY.md §0.4); norm2 / to_q /
+                    # to_k of attn2 cannot influence it and are packed only for a multi-token context (_pack_cross)
                     cv_w.append(sd[base + ".attn2.to_v.weight"])
                     cv_off[base] = (cv_total, c)
                     cv_total += c
@@ -675,6 +675,24 @@ class VideoUNet(KernelModule):
         P["cv_off"], P["cv_total"] = cv_off, cv_total
         P["pos_cache"] = {}
         return P
+
+    def _pack_cross(self, P: dict) -> None:
+        """The attn2 weights only a context of more than one token reads - norm2, to_q, and to_k | to_v of every layer
+        stacked into one [sum 2C, context_dim] matrix (layer `base` at rows P["ckv_off"][base][0]: its C K rows, then
+        its C V rows) - added to P on the first such forward, so the single-token path never allocates them."""
+        if "ckv_all.weight" in P:
+            return
+        sd = {k: v.detach() for k, v in self.named_parameters()}
+        kv_w, kv_off, total = [], {}, 0
+        for base, (_, c) in P["cv_off"].items():
+            kv_w += [sd[base + ".attn2.to_k.weight"], sd[base + ".attn2.to_v.weight"]]
+            kv_off[base] = (total, c)
+            total += 2 * c
+            P[base + ".attn2.to_q.weight"] = self._bf(sd[base + ".attn2.to_q.weight"])
+            P[base + ".norm2.weight"] = self._f32(sd[base + ".norm2.weight"])
+            P[base + ".norm2.bias"] = self._f32(sd[base + ".norm2.bias"])
+        P["ckv_off"] = kv_off
+        P["ckv_all.weight"] = self._bf(torch.cat(kv_w, 0))
 
     # ------------------------------------------------------------------------------------------
     # forward
@@ -718,16 +736,17 @@ class VideoUNet(KernelModule):
 
     def _prepare(self, x, timesteps, context, y, time_context, num_video_frames, image_only_indicator):
         """Argument checks of VideoUNet.forward (video_model.py:452-461) and assembly of the schedule's inputs:
-        -> ((x, timesteps, context rows, y) fp32 contiguous, (B, T, nb, H, W), use CUDA graphs)."""
+        -> ((x, timesteps, context rows, y) fp32 contiguous, (B, T, nb, H, W), use CUDA graphs).  The context rows are
+        [B (+ nb time-context rows when frame-sharded), M * context_dim]: one row per sample holding its M tokens."""
         assert (y is not None) == (self.num_classes is not None), \
             "must specify y if and only if the model is class-conditional"
         assert y is None or y.shape[0] == x.shape[0]
         assert context is not None and context.ndim == 3, \
             f"n dims of spatial context should be 3 but are {None if context is None else context.ndim}"
         assert num_video_frames, "num_video_frames is required"
-        if context.shape[1] != 1:
-            raise NotImplementedError("cross-attention context with more than one token is not implemented "
-                                      "(V3D conditions on a single CLIP image token)")
+        M = context.shape[1]
+        assert M >= 1 and context.shape[2] == self.context_dim, \
+            f"context must be [B, tokens >= 1, {self.context_dim}], got {tuple(context.shape)}"
         B, cin, H, W = x.shape
         T = int(num_video_frames)
         assert B % T == 0 and cin == self.in_channels
@@ -745,10 +764,10 @@ class VideoUNet(KernelModule):
         if vs is not None:
             # frame-sharded call: x / context / y hold this rank's T = vs.tl frames of each video; the temporal
             # cross-attention context (frame 0 of each video, video_attention.py:250) may live on another rank and
-            # arrives through `time_context` [nb, 1, ctx]; its rows are appended to the context matrix
+            # arrives through `time_context` [nb, M, ctx]; its rows are appended to the context matrix
             assert T == vs.tl, f"view-sharded forward expects this rank's {vs.tl} frames, got num_video_frames={T}"
-            assert time_context is not None and time_context.shape[0] == nb and time_context.ndim == 3, \
-                "view-sharded forward needs time_context = context of frame 0 of each video, [nb, 1, ctx]"
+            assert time_context is not None and time_context.ndim == 3 and time_context.shape[:2] == (nb, M), \
+                f"view-sharded forward needs time_context = context of frame 0 of each video, [nb, {M}, ctx]"
             ctx2d = torch.cat([ctx2d, time_context.float().reshape(nb, -1).to(dev)], dim=0)
             # the one-sided peer transport is stream-ordered kernels only: always capturable.  torch.distributed
             # collectives inside a captured graph stay opt-in (V3D_VIEWSHARD_GRAPH=1)
@@ -757,15 +776,16 @@ class VideoUNet(KernelModule):
         args = (x.float().contiguous(), timesteps.float().contiguous(), ctx2d.contiguous(), y.float().contiguous())
         return args, (B, T, nb, H, W), graphs
 
-    def _graph_key(self, B, T, H, W, dev) -> tuple:
-        """Cache key of a captured graph: the shape, the device, the shard and the deterministic mode (the two modes
-        launch different GroupNorm kernels, so a graph captured in one is never replayed in the other)."""
+    def _graph_key(self, B, T, H, W, dev, M: int = 1) -> tuple:
+        """Cache key of a captured graph: the shape, the context's token count M (a multi-token context runs another
+        schedule), the device, the shard and the deterministic mode (the two modes launch different GroupNorm kernels,
+        so a graph captured in one is never replayed in the other)."""
         vs = self.view_shard
         key = (B, T, H, W, dev.index) if vs is None else (B, T, H, W, dev.index, vs.num_frames, vs.rank, vs.world)
-        return key + (("deterministic",) if ops.deterministic() else ())
+        return key + (("deterministic",) if ops.deterministic() else ()) + ((("tokens", M),) if M != 1 else ())
 
     def _run_graphed(self, P, args, B, T, nb, H, W, dev):
-        key = self._graph_key(B, T, H, W, dev)
+        key = self._graph_key(B, T, H, W, dev, args[2].shape[1] // self.context_dim)
         entry = self._graphs.get(key)
         if entry is None:
             # first call with this shape runs eagerly: warms kernel attributes and the positional-embedding cache
@@ -803,6 +823,14 @@ class VideoUNet(KernelModule):
         # every ResBlock's emb_layers (SiLU -> Linear) in one launch: [B, sum(Cout)]
         emb_all = torch.empty(B, P["emb_total"], device=dev)
         ops.small_linear(emb, P["emb_all.weight"], P["emb_all.bias"], emb_all, act_in=ops.ACT_SILU)
+        ctx_dim = self.context_dim
+        if ctx2d.shape[1] > ctx_dim:
+            # multi-token context: K | V of every attn2 layer over all context rows ((B + time-context rows) * M) in
+            # one GEMM; the layers' attention reads its column slices in place
+            rows = ctx2d.numel() // ctx_dim
+            ctx_bf = torch.empty(rows, ctx_dim, device=dev, dtype=torch.bfloat16)
+            ops.nchw_f32_to_nhwc_bf16(ctx2d.view(1, 1, rows, ctx_dim), ctx_bf)       # C = 1: a plain bf16 conversion
+            return emb_all, self._linear(P, "ckv_all", ctx_bf, rows)
         # single-token cross-attention: v = to_v(ctx) for every layer in one launch, then to_out per layer
         nctx = ctx2d.shape[0]  # B, plus one time-context row per video when frame-sharded
         v_all = torch.empty(nctx, P["cv_total"], device=dev)
@@ -859,8 +887,11 @@ class VideoUNet(KernelModule):
         self._tconv(P, ts + ".out_layers.3", a, h2, hw, T, nb, cout, r1=xs, s1=1.0, s0=1.0 - alpha)
         return h2
 
-    def _attn_block(self, P, st: _Step, x, cross, B, T, nb, h, w):
-        """SpatialVideoTransformer.forward (video_attention.py:230-301) with depth 1."""
+    def _attn_block(self, P, st: _Step, x, cross, B, T, nb, h, w, M: int = 1):
+        """SpatialVideoTransformer.forward (video_attention.py:230-301) with depth 1.  M = context tokens.  With one
+        token, `cross` holds every layer's attn2 output (fp32 rows, folded into attn1.to_out's epilogue as a bias); with
+        more, it holds every layer's attn2 K | V rows (bf16, one row per context token) and attn2 runs on its own
+        (_cross_attn)."""
         nm, c = st.name, st.cin
         hw = h * w
         rows = B * hw
@@ -868,8 +899,9 @@ class VideoUNet(KernelModule):
         scale = 64 ** -0.5
         X = cross.shape[1]
         tb, ts = nm + ".transformer_blocks.0", nm + ".time_stack.0"
-        os_, _ = P["cv_off"][tb]
-        ot, _ = P["cv_off"][ts]
+        off = P["cv_off"] if M == 1 else P["ckv_off"]
+        os_, _ = off[tb]
+        ot, _ = off[ts]
         dev = x.device
 
         def ln(key, src, **kw):
@@ -883,8 +915,13 @@ class VideoUNet(KernelModule):
         qkv = self._linear(P, tb + ".attn1.qkv", a, rows)
         o = torch.empty(rows, c, device=dev, dtype=torch.bfloat16)
         ops.attention_spatial(qkv, o, B, hw, heads, scale)
-        self._linear(P, tb + ".attn1.to_out.0", o, rows, out=t, r1=t, s1=1.0,
-                     fbias=cross[:, os_:], ldfb=X, rows_per_frame=hw)          # + attn2 (single key) folded in
+        if M == 1:
+            self._linear(P, tb + ".attn1.to_out.0", o, rows, out=t, r1=t, s1=1.0,
+                         fbias=cross[:, os_:], ldfb=X, rows_per_frame=hw)          # + attn2 (single key) folded in
+        else:
+            self._linear(P, tb + ".attn1.to_out.0", o, rows, out=t, r1=t, s1=1.0)
+            # each frame attends to its own M context tokens (attention.py:571-572)
+            self._cross_attn(P, tb, t, o, a, cross[:, os_:os_ + 2 * c], B, hw, M, M)
         a = ln(tb + ".norm3", t)
         g = self._linear(P, tb + ".ff.net.0.proj", a, rows, act=ops.ACT_GEGLU)
         self._linear(P, tb + ".ff.net.2", g, rows, out=t, r1=t, s1=1.0)
@@ -906,11 +943,13 @@ class VideoUNet(KernelModule):
                            **({"kv": (c, kv_dst, 2 * c)} if kv_dst is not None else {}))
         if vs is None:
             ops.attention_temporal(qkv, o, nb, T, hw, heads, scale)
-            # temporal cross-attention context = context[::T] (video_attention.py:250): row b*T of `cross`
-            tc_bias, tc_ld = cross[:, ot:], X * T
+            # temporal cross-attention context = context[::T] (video_attention.py:250): the rows of frame 0 of each
+            # video, row b*T of `cross` (one token) or rows b*T*M .. b*T*M + M - 1 (M tokens)
+            tc0, tc_ld = 0, X * T
         else:
             # frame-sharded: all-gather the packed K|V rows of every rank's frames, attend in place through the
             # per-frame row table; the time context (global frame 0 of each CFG half) is rows B.. of `cross`
+            # (B*M.. with M tokens)
             if kv_dst is not None:
                 gathered = vs.gather_signal(kv_buf)
             else:
@@ -918,15 +957,30 @@ class VideoUNet(KernelModule):
                 gathered = vs.gather_rows(send, kv_buf, rows)
             kv_row, kv_bstride = vs.kv_table(nb, hw)
             ops.attention_temporal_kv(qkv, gathered, o, nb, T, hw, heads, kv_row, kv_bstride, scale)
-            tc_bias, tc_ld = cross[B:, ot:], X
-        self._linear(P, ts + ".attn1.to_out.0", o, rows, out=xm, r1=xm, s1=1.0,
-                     fbias=tc_bias, ldfb=tc_ld, rows_per_frame=T * hw)
+            tc0, tc_ld = B, X
+        if M == 1:
+            self._linear(P, ts + ".attn1.to_out.0", o, rows, out=xm, r1=xm, s1=1.0,
+                         fbias=cross[tc0:, ot:], ldfb=tc_ld, rows_per_frame=T * hw)
+        else:
+            self._linear(P, ts + ".attn1.to_out.0", o, rows, out=xm, r1=xm, s1=1.0)
+            kstride = T * M if vs is None else M
+            self._cross_attn(P, ts, xm, o, a, cross[tc0 * M:, ot:ot + 2 * c], nb, T * hw, M, kstride)
         a = ln(ts + ".norm3", xm)
         g = self._linear(P, ts + ".ff.net.0.proj", a, rows, out=g, act=ops.ACT_GEGLU)
         alpha = P[nm + ".alpha"]
         # x = alpha * x_spatial + (1 - alpha) * (ff(.) + x_mix)   (AlphaBlender, util.py:358-369)
         self._linear(P, ts + ".ff.net.2", g, rows, out=t, r1=xm, s1=1.0 - alpha, r2=t, s2=alpha, s0=1.0 - alpha)
         return self._linear(P, nm + ".proj_out", t, rows, out=xn, r1=x, s1=1.0)
+
+    def _cross_attn(self, P, base, x, qbuf, obuf, kv, nbatch, nq, M, kv_bstride):
+        """x += attn2(norm2(x), context) over a context of M > 1 tokens (attention.py:286-349): LayerNorm, to_q GEMM,
+        attention of item b's nq rows against the K | V rows `kv` [b * kv_bstride, + M), to_out GEMM with the residual
+        in its epilogue.  qbuf / obuf: [rows, C] scratch buffers."""
+        rows, c = x.shape
+        ops.layernorm(x, obuf, P[base + ".norm2.weight"], P[base + ".norm2.bias"], rows, c)
+        q = self._linear(P, base + ".attn2.to_q", obuf, rows, out=qbuf)
+        ops.attention_cross(q, kv, obuf, nbatch, nq, M, c // 64, 64 ** -0.5, kv_bstride=kv_bstride)
+        self._linear(P, base + ".attn2.to_out.0", obuf, rows, out=x, r1=x, s1=1.0)
 
     def _run(self, P, x, timesteps, ctx2d, y, B, T, nb, H, W, dev):
         if self.view_shard is not None:
@@ -939,6 +993,9 @@ class VideoUNet(KernelModule):
             object.__setattr__(self, "_gn_pool", None)
 
     def _run_inner(self, P, x, timesteps, ctx2d, y, B, T, nb, H, W, dev):
+        M = ctx2d.shape[1] // self.context_dim
+        if M > 1:
+            self._pack_cross(P)
         emb_all, cross = self._embeddings(P, timesteps, ctx2d, y, B, T, dev)
         cur = torch.empty(B * H * W, self.in_channels, device=dev, dtype=torch.bfloat16)
         ops.nchw_f32_to_nhwc_bf16(x, cur)
@@ -955,7 +1012,7 @@ class VideoUNet(KernelModule):
                 cur = self._res_block(P, st, cur, emb_all, B, T, nb, h, w)
                 ch = st.cout
             elif st.kind == "attn":
-                cur = self._attn_block(P, st, cur, cross, B, T, nb, h, w)
+                cur = self._attn_block(P, st, cur, cross, B, T, nb, h, w, M)
             elif st.kind == "down":
                 cur = self._conv3x3(P, st.name + ".op", cur, B, h, w, st.cin, stride=2)
                 h, w = (h + 2 - 3) // 2 + 1, (w + 2 - 3) // 2 + 1

@@ -579,7 +579,7 @@ class ViewShard:
 
     def time_context(self, c: Dict, uc: Dict) -> torch.Tensor:
         """The temporal cross-attention context is `context[::T]` = frame 0 of each CFG half
-        (video_attention.py:250): [2, 1, ctx] in [uc; c] order, the same on every rank."""
+        (video_attention.py:250): [2, M, ctx] in [uc; c] order (M context tokens), the same on every rank."""
         return torch.cat([uc["crossattn"][:1], c["crossattn"][:1]], dim=0).contiguous()
 
     def shard_guider(self, guider):

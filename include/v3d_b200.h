@@ -183,13 +183,17 @@ int v3d_attention_spatial(const void* q, const void* k, const void* v, void* o, 
 int v3d_attention_spatial_mma(const void* q, const void* k, const void* v, void* o, int64_t ld_qkv, int64_t ld_o,
                               int32_t nbatch, int32_t ntok, int32_t nheads, float scale, void* stream);
 /* the same attention across the T view-frames of each pixel (video_attention.py:114,125), reading the
- * frame-major token matrix in place: row(b,t,s) = (b*T + t)*S + s, T <= 32. */
+ * frame-major token matrix in place: row(b,t,s) = (b*T + t)*S + s, 1 <= T <= 128.  T <= 32 runs one warp per
+ * (pixel, head) sequence; 33..128 runs one CTA per sequence with the 16-query tiles split over its warps and a
+ * single-pass softmax over the whole key row (same arithmetic).  T > 128 is V3D_ERR_BAD_ARG: it would need an online
+ * softmax over key tiles. */
 int v3d_attention_temporal(const void* q, const void* k, const void* v, void* o, int64_t ld_qkv, int64_t ld_o,
                            int32_t nb, int32_t T, int32_t S, int32_t nheads, float scale, void* stream);
 /* frame-sharded form (SURVEY.md 8(e); the "temporal-attention KV all-gather" of BASELINE.json): q / o hold this rank's
  * Tq frames (row(b,t,s) = (b*Tq + t)*S + s); k / v point into the all-gathered K|V buffer (row stride ld_kv) where key
  * frame f of CFG half b, pixel s is row kv_row[f] + b*kv_bstride[f] + s (host int32[Tk] arrays, rank-major layout).
- * Tq <= Tk <= 32. */
+ * 1 <= Tq <= Tk <= 128; the kernel is chosen by Tk as v3d_attention_temporal chooses it by T, and gives the same bits as
+ * the dense form on the same rows. */
 int v3d_attention_temporal_kv(const void* q, const void* k, const void* v, void* o, int64_t ld_q, int64_t ld_kv,
                               int64_t ld_o, int32_t nb, int32_t Tq, int32_t Tk, int32_t S, int32_t nheads,
                               const int32_t* kv_row, const int32_t* kv_bstride, float scale, void* stream);

@@ -6,6 +6,7 @@
 //   temporal: sequences of T <= 32 view-frames per (pixel, head); one warp per sequence, whole
 //             problem on chip, no online softmax. Reads q/k/v with the frame stride directly from the
 //             frame-major token matrix, so "(b t) s c -> (b s) t c" is never materialised.
+//             32 < T <= 128: one CTA per sequence, warps split the query tiles (attn_temporal_long_kernel).
 #include <cstring>
 
 #include "common.cuh"
@@ -439,6 +440,188 @@ attn_temporal_kernel(const bf16* __restrict__ Q, const bf16* __restrict__ K, con
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// temporal attention over 32 < T <= 128 frames: grid = (pixels, heads, halves b), one (pixel, head) sequence per CTA.
+//
+// Why not the short kernel's "one warp owns a sequence": at T = 128 a sequence's Q, K and V tiles are 3 x 16 KB, so
+// four warp-private sequences would take 192 KB and leave one CTA of 4 warps per SM, far too few loads in flight for
+// a kernel that is bound by its HBM gathers.  Here the CTA's 4 warps share one K and one V tile and split the 16-query
+// m-tiles between them (warp w takes m-tiles w, w + 4): 48 KB at T = 128, 18 KB at T = 48, all within the 48 KB that
+// need no opt-in.  ptxas: 110 registers (KT = 8) and 82 (KT = 4), no spills, so 4 CTAs of 128 threads fit an SM by
+// registers and by shared memory even at T = 128 (4 x 48 KB), each with its whole gather in flight before its first
+// MMA; the launch bounds only keep the compiler from growing past 3 (KT = 8) / 4 (KT = 4) resident CTAs' worth.
+//
+// Per m-tile, a warp holds the complete score row block in registers (2 KT n-tiles x 4 fp32; Tk <= 128 so KT <= 8), so
+// the softmax is single-pass: S = Q K^T on mma.m16n8k16, keys >= Tk set to -inf, row maximum and sum by quad shuffles,
+// p = ex2(s * scale*log2e - max * scale*log2e), P packed to bf16 A fragments, O = P V, normalised in fp32.  KT is the
+// capacity in 16-key tiles (4: Tk <= 64, 8: Tk <= 128); 16-key tiles at or beyond the padded key count are skipped.
+// Rows are gathered with the frame stride by cp.async 16-byte chunks; rows of the last 16-row tile at or beyond T /
+// Tk are zero-filled by cp.async itself (source size 0), so 0 x garbage cannot occur.  Each warp stages its m-tile of
+// O through the Q rows it alone read and writes it back as 16-byte chunks.
+//
+// SPLIT: as in attn_temporal_kernel; the row table holds up to kMaxTLong key frames.
+// ------------------------------------------------------------------------------------------------
+constexpr int kMaxTLong = 128;
+constexpr int kTlWarps = 4;
+
+struct TaKVLong {
+  int tk;
+  int row[kMaxTLong];
+  int bstride[kMaxTLong];
+};
+
+template <bool SPLIT, int KT>
+__global__ void __launch_bounds__(kTlWarps * 32, KT == 4 ? 4 : 3)
+attn_temporal_long_kernel(const bf16* __restrict__ Q, const bf16* __restrict__ K, const bf16* __restrict__ V,
+                          bf16* __restrict__ O, long long ld, long long ldo, int T, int S, float scale_log2e,
+                          long long ldkv, const __grid_constant__ TaKVLong kv) {
+  extern __shared__ __align__(128) uint8_t tl_smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = lane >> 2, t = lane & 3;
+  const int s = blockIdx.x, b = blockIdx.z;
+  const long long col = static_cast<long long>(blockIdx.y) * HD;
+  const int TK = SPLIT ? kv.tk : T;                        // key / value frames
+  const int Tp = (T + 15) & ~15, TKp = (TK + 15) & ~15;    // rows of the Q tile / of the K and V tiles
+  uint8_t* sq = tl_smem;
+  uint8_t* sk = sq + Tp * 128;
+  uint8_t* sv = sk + TKp * 128;
+  const long long row_base = (static_cast<long long>(b) * T) * S + s;
+
+  for (int i = threadIdx.x; i < Tp * 8; i += kTlWarps * 32) {
+    const int r = i >> 3, c = i & 7;
+    const bool ok = r < T;
+    cp_async16(sq + tile_off(r, c), Q + (row_base + static_cast<long long>(ok ? r : 0) * S) * ld + col + c * 8, ok);
+  }
+  for (int i = threadIdx.x; i < TKp * 8; i += kTlWarps * 32) {
+    const int r = i >> 3, c = i & 7;
+    const bool ok = r < TK;
+    const int f = ok ? r : 0;
+    const long long row = SPLIT ? static_cast<long long>(kv.row[f]) + static_cast<long long>(b) * kv.bstride[f] + s
+                                : row_base + static_cast<long long>(f) * S;
+    const long long off = row * ldkv + col + c * 8;
+    cp_async16(sk + tile_off(r, c), K + off, ok);
+    cp_async16(sv + tile_off(r, c), V + off, ok);
+  }
+  cp_async_commit();
+  cp_async_wait<0>();
+  __syncthreads();
+
+  const int mi = lane >> 3;
+  for (int m0 = warp * 16; m0 < Tp; m0 += kTlWarps * 16) {
+    // ---- S = Q K^T for this warp's 16 queries
+    uint32_t qa[4][4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+      ldsm_x4(smem_u32(sq + tile_off(m0 + (lane & 15), kk * 2 + (lane >> 4))), qa[kk][0], qa[kk][1], qa[kk][2],
+              qa[kk][3]);
+    float sc[2 * KT][4];
+#pragma unroll
+    for (int j = 0; j < 2 * KT; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) sc[j][e] = 0.f;
+#pragma unroll
+    for (int jp = 0; jp < KT; ++jp) {  // pairs of key n-tiles
+      if (jp * 16 < TKp) {
+        const int key = jp * 16 + (mi >> 1) * 8 + (lane & 7);
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+          uint32_t b0, b1, b2, b3;
+          ldsm_x4(smem_u32(sk + tile_off(key, kk * 2 + (mi & 1))), b0, b1, b2, b3);
+          mma_bf16_16816(sc[2 * jp], qa[kk], b0, b1);
+          mma_bf16_16816(sc[2 * jp + 1], qa[kk], b2, b3);
+        }
+      }
+    }
+    // ---- softmax over keys, rows g / g+8; P packed as A fragments
+    float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+    for (int j = 0; j < 2 * KT; ++j) {
+      const int key = j * 8 + 2 * t;
+      if (key >= TK) { sc[j][0] = -INFINITY; sc[j][2] = -INFINITY; }
+      if (key + 1 >= TK) { sc[j][1] = -INFINITY; sc[j][3] = -INFINITY; }
+      mx0 = fmaxf(mx0, fmaxf(sc[j][0], sc[j][1]));
+      mx1 = fmaxf(mx1, fmaxf(sc[j][2], sc[j][3]));
+    }
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+    const float m0s = mx0 * scale_log2e, m1s = mx1 * scale_log2e;
+    float s0 = 0.f, s1 = 0.f;
+    uint32_t pf[KT][4];
+#pragma unroll
+    for (int j = 0; j < 2 * KT; ++j) {
+      const float p0 = ex2_approx(fmaf(sc[j][0], scale_log2e, -m0s));
+      const float p1 = ex2_approx(fmaf(sc[j][1], scale_log2e, -m0s));
+      const float p2 = ex2_approx(fmaf(sc[j][2], scale_log2e, -m1s));
+      const float p3 = ex2_approx(fmaf(sc[j][3], scale_log2e, -m1s));
+      s0 += p0 + p1;
+      s1 += p2 + p3;
+      pf[j >> 1][(j & 1) * 2] = pack_bf16x2(p0, p1);
+      pf[j >> 1][(j & 1) * 2 + 1] = pack_bf16x2(p2, p3);
+    }
+    s0 += __shfl_xor_sync(0xffffffffu, s0, 1);
+    s0 += __shfl_xor_sync(0xffffffffu, s0, 2);
+    s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
+    s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
+    const float inv0 = 1.f / s0, inv1 = 1.f / s1;
+    // ---- O = P V
+    float oc[8][4];
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) oc[j][e] = 0.f;
+#pragma unroll
+    for (int kk = 0; kk < KT; ++kk) {
+      if (kk * 16 < TKp) {
+        const int key = kk * 16 + (mi & 1) * 8 + (lane & 7);
+#pragma unroll
+        for (int jp = 0; jp < 4; ++jp) {  // pairs of d n-tiles
+          uint32_t b0, b1, b2, b3;
+          ldsm_x4_t(smem_u32(sv + tile_off(key, jp * 2 + (mi >> 1))), b0, b1, b2, b3);
+          mma_bf16_16816(oc[2 * jp], pf[kk], b0, b1);
+          mma_bf16_16816(oc[2 * jp + 1], pf[kk], b2, b3);
+        }
+      }
+    }
+    // ---- stage O (normalised, bf16) through this warp's Q rows, then 16-byte row-chunk stores of the rows < T
+    __syncwarp();
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int colb = (j * 8 + 2 * t) * 2;  // byte offset inside the 128-byte row
+      *reinterpret_cast<uint32_t*>(sq + tile_off(m0 + g, colb >> 4) + (colb & 15)) =
+          pack_bf16x2(oc[j][0] * inv0, oc[j][1] * inv0);
+      *reinterpret_cast<uint32_t*>(sq + tile_off(m0 + g + 8, colb >> 4) + (colb & 15)) =
+          pack_bf16x2(oc[j][2] * inv1, oc[j][3] * inv1);
+    }
+    __syncwarp();
+    for (int i = lane; i < 16 * 8; i += 32) {
+      const int r = m0 + (i >> 3), c = i & 7;
+      if (r < T)
+        *reinterpret_cast<uint4*>(O + (row_base + static_cast<long long>(r) * S) * ldo + col + c * 8) =
+            *reinterpret_cast<const uint4*>(sq + tile_off(r, c));
+    }
+  }
+}
+
+// Host side of both temporal entry points for 32 < Tk <= 128.
+template <bool SPLIT>
+static void launch_temporal_long(const void* q, const void* k, const void* v, void* o, int64_t ld_q, int64_t ld_kv,
+                                 int64_t ld_o, int nb, int Tq, int S, int nheads, float scale, const TaKVLong& kv,
+                                 cudaStream_t st) {
+  const int smem = (((Tq + 15) & ~15) + 2 * ((kv.tk + 15) & ~15)) * 128;   // <= 48 KB: no opt-in needed
+  dim3 grid(S, nheads, nb);
+  const float sl2 = scale * 1.44269504088896340736f;
+  if (kv.tk <= 64)
+    attn_temporal_long_kernel<SPLIT, 4><<<grid, kTlWarps * 32, smem, st>>>(
+        static_cast<const bf16*>(q), static_cast<const bf16*>(k), static_cast<const bf16*>(v),
+        static_cast<bf16*>(o), ld_q, ld_o, Tq, S, sl2, ld_kv, kv);
+  else
+    attn_temporal_long_kernel<SPLIT, 8><<<grid, kTlWarps * 32, smem, st>>>(
+        static_cast<const bf16*>(q), static_cast<const bf16*>(k), static_cast<const bf16*>(v),
+        static_cast<bf16*>(o), ld_q, ld_o, Tq, S, sl2, ld_kv, kv);
+}
+
 }  // namespace v3d
 
 using namespace v3d;
@@ -487,12 +670,21 @@ int v3d_attention_spatial_mma(const void* q, const void* k, const void* v, void*
  * attention.py:337-341), on the frame-major token matrix: row(b,t,s) = (b*T + t)*S + s. */
 int v3d_attention_temporal(const void* q, const void* k, const void* v, void* o, int64_t ld_qkv, int64_t ld_o,
                            int32_t nb, int32_t T, int32_t S, int32_t nheads, float scale, void* stream) {
-  if (!q || !k || !v || !o || ld_qkv % 8 != 0 || ld_o % 8 != 0 || T <= 0 || T > kMaxT || nheads <= 0 ||
-      nb <= 0 || nb > 65535 || S <= 0) {
-    set_error("v3d_attention_temporal: bad args (T=%d must be <= %d)", T, kMaxT);
+  if (!q || !k || !v || !o || ld_qkv % 8 != 0 || ld_o % 8 != 0 || T <= 0 || T > kMaxTLong || nheads <= 0 ||
+      nheads > 65535 || nb <= 0 || nb > 65535 || S <= 0) {
+    set_error("v3d_attention_temporal: bad args (T=%d must be 1..%d: a longer sequence needs an online softmax over "
+              "key tiles, which this kernel family does not have)", T, kMaxTLong);
     return V3D_ERR_BAD_ARG;
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (T > kMaxT) {
+    TaKVLong none;
+    memset(&none, 0, sizeof(none));
+    none.tk = T;
+    launch_temporal_long<false>(q, k, v, o, ld_qkv, ld_qkv, ld_o, nb, T, S, nheads, scale, none, st);
+    V3D_CHECK_LAUNCH("attn_temporal_long_kernel");
+    return V3D_OK;
+  }
   const int smem = kTaWarps * 3 * kTaTile;
   dim3 grid(S, nb);
   TaKV none;
@@ -515,9 +707,27 @@ int v3d_attention_temporal_kv(const void* q, const void* k, const void* v, void*
                               int64_t ld_o, int32_t nb, int32_t Tq, int32_t Tk, int32_t S, int32_t nheads,
                               const int32_t* kv_row, const int32_t* kv_bstride, float scale, void* stream) {
   if (!q || !k || !v || !o || !kv_row || !kv_bstride || ld_q % 8 != 0 || ld_kv % 8 != 0 || ld_o % 8 != 0 ||
-      Tq <= 0 || Tq > Tk || Tk > kMaxT || nheads <= 0 || nb <= 0 || nb > 65535 || S <= 0) {
-    set_error("v3d_attention_temporal_kv: bad args (Tq=%d Tk=%d, need 0 < Tq <= Tk <= %d)", Tq, Tk, kMaxT);
+      Tq <= 0 || Tq > Tk || Tk > kMaxTLong || nheads <= 0 || nheads > 65535 || nb <= 0 || nb > 65535 || S <= 0) {
+    set_error("v3d_attention_temporal_kv: bad args (Tq=%d Tk=%d, need 0 < Tq <= Tk <= %d: more key frames need an "
+              "online softmax over key tiles, which this kernel family does not have)", Tq, Tk, kMaxTLong);
     return V3D_ERR_BAD_ARG;
+  }
+  if (Tk > kMaxT) {
+    TaKVLong kvl;
+    memset(&kvl, 0, sizeof(kvl));
+    kvl.tk = Tk;
+    for (int f = 0; f < Tk; ++f) {
+      if (kv_row[f] < 0 || kv_bstride[f] < 0) {
+        set_error("v3d_attention_temporal_kv: negative row offset for key frame %d", f);
+        return V3D_ERR_BAD_ARG;
+      }
+      kvl.row[f] = kv_row[f];
+      kvl.bstride[f] = kv_bstride[f];
+    }
+    launch_temporal_long<true>(q, k, v, o, ld_q, ld_kv, ld_o, nb, Tq, S, nheads, scale, kvl,
+                               static_cast<cudaStream_t>(stream));
+    V3D_CHECK_LAUNCH("attn_temporal_long_kernel<split>");
+    return V3D_OK;
   }
   TaKV kv;
   memset(&kv, 0, sizeof(kv));

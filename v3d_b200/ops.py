@@ -279,6 +279,16 @@ def attention_spatial_mma(qkv: torch.Tensor, out: torch.Tensor, nbatch: int, nto
     return out
 
 
+MAX_TEMPORAL_FRAMES = 128   # key frames v3d_attention_temporal / _kv take (kMaxTLong, csrc/attention.cu)
+
+
+def check_temporal_frames(num_frames: int) -> None:
+    """Raise before a schedule starts if the video has more view-frames than the temporal attention kernels hold in
+    one pass (longer sequences would need an online softmax over key tiles)."""
+    if num_frames > MAX_TEMPORAL_FRAMES:
+        raise ValueError(f"temporal attention supports at most {MAX_TEMPORAL_FRAMES} frames, got {num_frames}")
+
+
 def attention_temporal(qkv: torch.Tensor, out: torch.Tensor, nb: int, t: int, s: int, nheads: int,
                        scale: float) -> torch.Tensor:
     _need(qkv, torch.bfloat16, "attention qkv")

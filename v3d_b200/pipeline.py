@@ -1,7 +1,8 @@
 """The steps of `sample_one` either side of the hot path (scripts/pub/V3D_512.py:235-306; SURVEY.md 8(f)-1/-2), composed
 from the drop-in pieces: first-stage encode of the conditioning image, conditioning-augmentation noise, conditioner +
-per-frame repeat, latent noise, sampler loop + decode, uint8 wire format.  The CLIP image embedding is an INPUT (the
-ViT-H tower is out of scope; its output is [1, k, 1024]: one token per image, or k with n_cond_frames = k).
+per-frame repeat, latent noise, sampler loop + decode, uint8 wire format.  The CLIP image embedding is an INPUT of these
+functions ([1, k, 1024]: one token per image, or k with n_cond_frames = k); the native ViT-H/14 image tower that
+produces it is v3d_b200.clip.
 
 Random draws happen in the reference's order and on the reference's generators, so that with the same
 `torch.manual_seed(seed)` (V3D_512.py:177) a run reproduces the reference's noise: posterior sample of the encoder on

@@ -756,10 +756,11 @@ class VideoUNet(KernelModule):
             raise RuntimeError(f"latent size {H}x{W} must be divisible by {down}: the skip connections of the "
                                f"{len(self.channel_mult)}-level U-Net would not line up")
         nb = B // T
+        vs = self.view_shard
+        ops.check_temporal_frames(T if vs is None else vs.num_frames)   # keys = the whole video, also when sharded
         self._check_indicator(image_only_indicator, nb, T)
         dev = x.device
         ctx2d = context.float().reshape(B, -1)
-        vs = self.view_shard
         graphs = self.cuda_graphs
         if vs is not None:
             # frame-sharded call: x / context / y hold this rank's T = vs.tl frames of each video; the temporal

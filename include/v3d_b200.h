@@ -294,6 +294,32 @@ int v3d_decode_to_u8(const void* x, int64_t ldx, int32_t src_fp32, void* y, int6
 int v3d_frames_nchw_to_u8(const void* x, void* y, int32_t T, int64_t HW, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * PixelNeRF scene conditioning (pixelnerf.cu): the PixelNeRFEmbedder of sparse-view scene generation
+ * (sgm/modules/encoders/pixelnerf.py, math_utils.py).  Three launches: rays, the fused per-sample render (the
+ * feature MLP on wgmma, online softmax over the sample axis) and the per-ray decoder MLP.  MLP weights are bf16
+ * row-major [out][in] with zero padding: w1 [128][64 * ceil(d_in / 64)], w2 [128][128], w3 [136][128] (129 / 131 real
+ * rows); biases fp32, b3 [136].
+ * ------------------------------------------------------------------------------------------ */
+#define V3D_PNERF_STD 1        /* append the unbiased std over sources (zeros when S = 1) */
+#define V3D_PNERF_POSENC 2     /* append the 39-value NeRF positional encoding of the world sample */
+#define V3D_PNERF_NEAREST 4    /* grid_sample mode "nearest" (default "bilinear") */
+#define V3D_PNERF_ZEROS 8      /* grid_sample padding "zeros" (default "border") */
+#define V3D_PNERF_DISPARITY 16 /* disparity sampling: jitter holds z[ns], depth = 1 / (inv_near (1 - z) + inv_far z) */
+/* cams [ncam][25] -> rays [ncam * rs^2][8] = (origin, direction, t_start, t_end); limits: 2 words of scratch. */
+int v3d_pixelnerf_rays(const void* cams, int32_t ncam, int32_t render_size, float box_half, int32_t box, void* rays,
+                       void* limits, void* stream);
+/* rays + limits from v3d_pixelnerf_rays; jitter [ns][nrays] uniforms (box mode); src [B][S][C][H][W] fp32;
+ * src_w2c [B][S][3][4]; src_k [B][S][4] = (fx, fy, cx, cy); feat out [nrays][128] fp32.  ns >= 2, d_in <= 192. */
+int v3d_pixelnerf_render(const void* rays, const void* limits, const void* jitter, const void* src, const void* src_w2c,
+                         const void* src_k, int64_t nrays, int64_t rays_per_batch, int32_t S, int32_t C, int32_t H,
+                         int32_t W, int32_t ns, int32_t flags, float inv_near, float inv_far, const void* w1,
+                         int32_t d_in, const void* b1, const void* w2, const void* b2, const void* w3, const void* b3,
+                         void* feat, void* stream);
+/* feat [nrays][128] -> rgb [nrays / hw][3][hw] (sigmoid) and feats [nrays / hw][128][hw], fp32. */
+int v3d_pixelnerf_decode(const void* feat, int64_t nrays, int64_t hw, const void* w1, const void* b1, const void* w2,
+                         const void* b2, const void* w3, const void* b3, void* rgb, void* feats, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * One-sided exchanges over NVLink peer memory (peer.cu): the transport of the frame-sharded path - ONE image over
  * several GPUs of a box (BASELINE.json north_star; SURVEY.md 8(e)).  They replace, on the data path, the three
  * torch.distributed exchanges that the reference's single-GPU modules imply once the T frames are split over ranks:

@@ -107,6 +107,11 @@ SIGNATURES = {
                                _i32, _i64, _vp]),
     "v3d_decode_to_u8": (C.c_int, [_vp, _i64, _i32, _vp, _i64, _vp]),
     "v3d_frames_nchw_to_u8": (C.c_int, [_vp, _vp, _i32, _i64, _vp]),
+    # pixelnerf.cu
+    "v3d_pixelnerf_rays": (C.c_int, [_vp, _i32, _i32, _f32, _i32, _vp, _vp, _vp]),
+    "v3d_pixelnerf_render": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _i32,
+                                       _f32, _f32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "v3d_pixelnerf_decode": (C.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
 }
 
 

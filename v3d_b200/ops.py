@@ -519,3 +519,91 @@ def frames_nchw_to_u8(x: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
     _lib.check(_lib.load().v3d_frames_nchw_to_u8(x.data_ptr(), y.data_ptr(), t, h * w, _stream()),
                "v3d_frames_nchw_to_u8")
     return y
+
+
+PNERF_STD, PNERF_POSENC, PNERF_NEAREST, PNERF_ZEROS, PNERF_DISPARITY = 1, 2, 4, 8, 16
+
+
+def _need_contig(name: str, dtype, **ts) -> None:
+    for k, t in ts.items():
+        _need(t, dtype, f"{name} {k}")
+        if not t.is_contiguous():
+            raise RuntimeError(f"{name} {k}: expected a contiguous tensor")
+
+
+def pixelnerf_rays(cams: torch.Tensor, render_size: int, rays: torch.Tensor, limits: torch.Tensor,
+                   box: bool = True, box_half: float = 1.0) -> torch.Tensor:
+    """cams [ncam, 25] -> rays [ncam * render_size**2, 8] (origin, direction, t_start, t_end); limits: int32 [2]."""
+    _need_contig("pixelnerf_rays", torch.float32, cams=cams, rays=rays)
+    _need(limits, torch.int32, "pixelnerf_rays limits")
+    ncam = cams.numel() // 25
+    if cams.numel() != ncam * 25 or ncam == 0 or rays.numel() != ncam * render_size * render_size * 8 \
+            or limits.numel() < 2:
+        raise RuntimeError(f"pixelnerf_rays: cams {tuple(cams.shape)} / rays {tuple(rays.shape)} / limits "
+                           f"{tuple(limits.shape)} do not match [ncam, 25] / [ncam * {render_size}^2, 8] / [2]")
+    _lib.check(_lib.load().v3d_pixelnerf_rays(cams.data_ptr(), ncam, render_size, box_half, int(box), rays.data_ptr(),
+                                              limits.data_ptr(), _stream()), "v3d_pixelnerf_rays")
+    return rays
+
+
+def _mlp_shapes(name: str, mlp, k1: int) -> None:
+    w1, b1, w2, b2, w3, b3 = mlp
+    want = ((w1, (128, k1)), (b1, (128,)), (w2, (128, 128)), (b2, (128,)), (w3, (136, 128)), (b3, (136,)))
+    for i, (t, shape) in enumerate(want):
+        if tuple(t.shape) != shape:
+            raise RuntimeError(f"{name}: packed MLP tensor {i} is {tuple(t.shape)}, expected {shape}")
+
+
+def pixelnerf_render(rays, limits, jitter, src, src_w2c, src_k, rays_per_batch: int, ns: int, flags: int,
+                     inv_near: float, inv_far: float, mlp, d_in: int, feat: torch.Tensor) -> torch.Tensor:
+    """src [B, S, C, H, W] fp32; src_w2c [B, S, 3, 4]; src_k [B, S, 4]; mlp = (w1, b1, w2, b2, w3, b3) packed as
+    include/v3d_b200.h describes; feat out [nrays, 128] fp32.  Every shape relation the kernel relies on is checked
+    here: the kernel indexes by them without bounds checks."""
+    w1, b1, w2, b2, w3, b3 = mlp
+    _need_contig("pixelnerf_render", torch.float32, rays=rays, jitter=jitter, src=src, src_w2c=src_w2c, src_k=src_k,
+                 b1=b1, b2=b2, b3=b3, feat=feat)
+    _need_contig("pixelnerf_render", torch.bfloat16, w1=w1, w2=w2, w3=w3)
+    _need(limits, torch.int32, "pixelnerf_render limits")
+    if src.dim() != 5:
+        raise RuntimeError(f"pixelnerf_render: src must be [B, S, C, H, W], got {tuple(src.shape)}")
+    B, S, Cc, H, W = src.shape
+    nrays = rays.shape[0]
+    if rays.shape != (nrays, 8) or limits.numel() < 2:
+        raise RuntimeError("pixelnerf_render: rays must be [nrays, 8] and limits hold 2 words")
+    if rays_per_batch <= 0 or B * rays_per_batch != nrays:
+        raise RuntimeError(f"pixelnerf_render: {B} source batches x {rays_per_batch} rays != {nrays} rays "
+                           "(the sources' batch must equal the target cameras' batch)")
+    if tuple(src_w2c.shape) != (B, S, 3, 4) or tuple(src_k.shape) != (B, S, 4):
+        raise RuntimeError(f"pixelnerf_render: src_w2c {tuple(src_w2c.shape)} / src_k {tuple(src_k.shape)} do not "
+                           f"match [B={B}, S={S}, 3, 4] / [B, S, 4]")
+    want_j = ns if flags & PNERF_DISPARITY else ns * nrays
+    if jitter.numel() != want_j:
+        raise RuntimeError(f"pixelnerf_render: jitter has {jitter.numel()} values, expected {want_j}")
+    _mlp_shapes("pixelnerf_render", mlp, -(-d_in // 64) * 64)
+    if tuple(feat.shape) != (nrays, 128):
+        raise RuntimeError(f"pixelnerf_render: feat is {tuple(feat.shape)}, expected ({nrays}, 128)")
+    _lib.check(_lib.load().v3d_pixelnerf_render(
+        rays.data_ptr(), limits.data_ptr(), jitter.data_ptr(), src.data_ptr(), src_w2c.data_ptr(), src_k.data_ptr(),
+        nrays, rays_per_batch, S, Cc, H, W, ns, flags, inv_near, inv_far, w1.data_ptr(), d_in, b1.data_ptr(),
+        w2.data_ptr(), b2.data_ptr(), w3.data_ptr(), b3.data_ptr(), feat.data_ptr(), _stream()),
+        "v3d_pixelnerf_render")
+    return feat
+
+
+def pixelnerf_decode(feat: torch.Tensor, hw: int, mlp, rgb: torch.Tensor, feats: torch.Tensor):
+    """feat [nrays, 128] -> rgb [nrays / hw, 3, hw] (sigmoid), feats [nrays / hw, 128, hw]."""
+    w1, b1, w2, b2, w3, b3 = mlp
+    _need_contig("pixelnerf_decode", torch.float32, feat=feat, b1=b1, b2=b2, b3=b3, rgb=rgb, feats=feats)
+    _need_contig("pixelnerf_decode", torch.bfloat16, w1=w1, w2=w2, w3=w3)
+    nrays = feat.shape[0]
+    if feat.dim() != 2 or feat.shape[1] != 128 or hw <= 0 or nrays % hw != 0:
+        raise RuntimeError(f"pixelnerf_decode: feat {tuple(feat.shape)} is not [n * {hw}, 128]")
+    n = nrays // hw
+    if rgb.numel() != n * 3 * hw or feats.numel() != n * 128 * hw:
+        raise RuntimeError(f"pixelnerf_decode: rgb {tuple(rgb.shape)} / feats {tuple(feats.shape)} do not hold "
+                           f"[{n}, 3, {hw}] / [{n}, 128, {hw}]")
+    _mlp_shapes("pixelnerf_decode", mlp, 128)
+    _lib.check(_lib.load().v3d_pixelnerf_decode(feat.data_ptr(), nrays, hw, w1.data_ptr(), b1.data_ptr(),
+                                                w2.data_ptr(), b2.data_ptr(), w3.data_ptr(), b3.data_ptr(),
+                                                rgb.data_ptr(), feats.data_ptr(), _stream()), "v3d_pixelnerf_decode")
+    return rgb, feats

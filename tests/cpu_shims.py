@@ -3,13 +3,13 @@
 The product classes refuse non-CUDA tensors in `forward` / `__call__` (there is no CPU path).  These subclasses skip
 exactly that check and call the same `_prepare` / `_run` / `_loop` the product path calls next, so that - with
 tests/emu_ops.py patched over `v3d_b200.ops` - a whole `DiffusionEngine.sample_views` executes on a box without a GPU.
-Used by tests/test_host_schedule_cpu.py only.
 """
 import torch
 
 from v3d_b200.decoder import VideoDecoder
 from v3d_b200.encoder import Encoder
-from v3d_b200.sampling import EulerEDMSampler, HeunEDMSampler
+from v3d_b200.sampling import (DPMPP2MSampler, DPMPP2SAncestralSampler, EulerAncestralSampler, EulerEDMSampler,
+                               HeunEDMSampler, LinearMultistepSampler)
 from v3d_b200.unet import VideoUNet
 
 CPU = torch.device("cpu")
@@ -51,9 +51,31 @@ class CpuHeun(HeunEDMSampler):
     __call__ = HeunEDMSampler._loop
 
 
+class CpuEulerAncestral(EulerAncestralSampler):
+    __call__ = EulerAncestralSampler._loop
+
+
+class CpuDPMPP2SAncestral(DPMPP2SAncestralSampler):
+    __call__ = DPMPP2SAncestralSampler._loop
+
+
+class CpuDPMPP2M(DPMPP2MSampler):
+    __call__ = DPMPP2MSampler._loop
+
+
+class CpuLMS(LinearMultistepSampler):
+    __call__ = LinearMultistepSampler._loop
+
+
+CPU_SHIMS = {"EulerEDMSampler": CpuEuler, "HeunEDMSampler": CpuHeun, "EulerAncestralSampler": CpuEulerAncestral,
+             "DPMPP2SAncestralSampler": CpuDPMPP2SAncestral, "DPMPP2MSampler": CpuDPMPP2M,
+             "LinearMultistepSampler": CpuLMS}
+
+
 def cpu_engine(num_frames: int, num_steps: int, min_cfg: float = 1.5, max_cfg: float = 3.5, width: int = 64,
-               sampler_cls=CpuEuler):
-    """The smoke-sized V3D_512 engine (model_channels / decoder ch = `width`) with seeded weights, on CPU shims."""
+               sampler: str = "EulerEDMSampler"):
+    """The smoke-sized V3D_512 engine (model_channels / decoder ch = `width`) with seeded weights, on CPU shims; its
+    sampler is the CPU shim of `sampler` with V3D_512's schedule and guider."""
     from oracle import synth
     from v3d_b200 import engine
 
@@ -66,5 +88,6 @@ def cpu_engine(num_frames: int, num_steps: int, min_cfg: float = 1.5, max_cfg: f
     sd_d = synth.synth_state_dict(dec.param_shapes(), seed=12)
     unet.load_state_dict(sd_u, strict=True)
     dec.load_state_dict(sd_d, strict=True)
-    unet.__class__, dec.__class__, eng.sampler.__class__ = CpuUNet, CpuDecoder, sampler_cls
+    unet.__class__, dec.__class__ = CpuUNet, CpuDecoder
+    eng.sampler = CPU_SHIMS[sampler](**cfg["sampler_config"]["params"])
     return eng, sd_u, sd_d

@@ -1,5 +1,5 @@
 """Cross-attention over contexts of more than one token (the M > 1 schedule of VideoUNet), on CPU with the kernels'
-stand-ins (tests/emu_ops.py, and tests/cross_standins.py for v3d_attention_cross):
+stand-ins (tests/emu_ops.py):
 
   * the stand-in of v3d_attention_cross against an fp64 softmax attention written out by hand, over the key counts and
     key-set strides the GPU edge test runs;
@@ -45,48 +45,12 @@ def _cos(a, b):
     return (a @ b / (a.norm() * b.norm()).clamp_min(1e-12)).item()
 
 
-def _describe(v):
-    if isinstance(v, torch.Tensor):
-        return ("T", tuple(v.shape), str(v.dtype), tuple(v.stride()))
-    if isinstance(v, (list, tuple)):
-        return tuple(_describe(e) for e in v)
-    if isinstance(v, float):
-        return round(v, 9)
-    return v
-
-
-def launch_sequence(run):
-    """Run `run()` under the stand-ins and record every ops call: [(name, args, kwargs)] with tensors as shapes."""
-    import cross_standins
-    from v3d_b200 import ops
-
-    calls = []
-    with cross_standins.patched():
-        saved = {}
-        for n in cross_standins.EMULATED:
-            if n in ("launch_count", "groupnorm_workspace"):
-                continue
-            f = getattr(ops, n)
-            saved[n] = f
-
-            def rec(*a, _n=n, _f=f, **kw):
-                calls.append((_n, _describe(a), tuple(sorted((k, _describe(v)) for k, v in kw.items()))))
-                return _f(*a, **kw)
-
-            setattr(ops, n, rec)
-        try:
-            out = run()
-        finally:
-            for n, f in saved.items():
-                setattr(ops, n, f)
-    return out, calls
-
-
 def _digest(calls):
     return hashlib.sha256(repr(calls).encode()).hexdigest()
 
 
 def _single_token_forward():
+    import emu_ops
     from oracle import synth
     from v3d_b200.unet import VideoUNet
 
@@ -99,16 +63,15 @@ def _single_token_forward():
     y = torch.cat([uc["vector"], c["vector"]])
     ts = torch.linspace(-0.5, 1.2, 2 * T)
 
-    def run():
-        with torch.no_grad():
-            P = net._pack(torch.device("cpu"))
-            return net._run(P, xin, ts, ctx.reshape(2 * T, -1), y, 2 * T, T, 2, hw, hw, torch.device("cpu"))
-
-    return launch_sequence(run)
+    calls = []
+    with emu_ops.patched(calls), torch.no_grad():
+        P = net._pack(torch.device("cpu"))
+        net._run(P, xin, ts, ctx.reshape(2 * T, -1), y, 2 * T, T, 2, hw, hw, torch.device("cpu"))
+    return calls
 
 
 def test_single_token_forward_launch_sequence_is_unchanged():
-    _, calls = _single_token_forward()
+    calls = _single_token_forward()
     print("single-token forward:", len(calls), "ops calls, digest", _digest(calls))
     assert len(calls) == SINGLE_TOKEN_LAUNCHES
     assert _digest(calls) == SINGLE_TOKEN_DIGEST
@@ -153,13 +116,13 @@ def cross_operands(nbatch, nq, nk, nheads, gap, seed=0, amp=1.0, device="cpu"):
 @pytest.mark.parametrize("nk", [1, 2, 63, 64, 65, 77, 257])
 @pytest.mark.parametrize("gap", [0, 3])
 def test_attention_cross_standin_matches_fp64(nk, gap):
-    import cross_standins
+    import emu_ops
 
     nbatch, nq, nheads = 3, 37, 2
     c = nheads * 64
     q, kv, obuf, bs = cross_operands(nbatch, nq, nk, nheads, gap, seed=nk, amp=4.0)
     out = obuf[:, 24:24 + c]
-    cross_standins.attention_cross(q, kv, out, nbatch, nq, nk, nheads, 64 ** -0.5, kv_bstride=bs)
+    emu_ops.attention_cross(q, kv, out, nbatch, nq, nk, nheads, 64 ** -0.5, kv_bstride=bs)
     ref = cross_reference(q, kv, nbatch, nq, nk, nheads, 64 ** -0.5, bs)
     assert torch.isfinite(out.float()).all()
     assert ((out.double() - ref).abs() <= 2.0 ** -8 * ref.abs()).all()                # fp64, one bf16 rounding
@@ -197,7 +160,6 @@ CTX_TAP_TOL = 2.5e-2
 def test_unet_multi_token_schedule_matches_reference_golden(tag):
     """Output and block taps of the M-token schedule against the real reference (output rel-L2 3e-2 / cosine 0.999 for
     the whole tensor and every sample, like the single-token fixtures; taps CTX_TAP_TOL)."""
-    import cross_standins
     import emu_ops
     from oracle import synth
     from v3d_b200.unet import VideoUNet
@@ -209,7 +171,7 @@ def test_unet_multi_token_schedule_matches_reference_golden(tag):
     taps = {k[4:]: None for k in gold if k.startswith("tap:")}
     net.debug_taps = taps
     B, _, H, W = xin.shape
-    with cross_standins.patched(), torch.no_grad():
+    with emu_ops.patched(), torch.no_grad():
         n0 = emu_ops.launch_count()
         out = net.eval()._run(net._pack(torch.device("cpu")), xin, ts, ctx.reshape(B, -1), y, B, T, B // T, H, W,
                               torch.device("cpu"))
@@ -227,6 +189,7 @@ def test_duplicated_tokens_match_single_token_golden():
     """Softmax over M copies of one key is that key: the M-token schedule fed the single-token fixture's context
     repeated twice must meet that fixture's own bounds (taps 2e-2, output 3e-2 / 0.999), through norm2, to_q, the
     attention kernel's stand-in, to_out and the frame-0 key sets of the temporal attn2."""
+    import emu_ops
     from oracle import synth
     from v3d_b200.unet import VideoUNet
 
@@ -242,8 +205,10 @@ def test_duplicated_tokens_match_single_token_golden():
     y = torch.cat([uc["vector"], c["vector"]])
     taps = {k[4:]: None for k in gold if k.startswith("tap:")}
     net.debug_taps = taps
-    out, calls = launch_sequence(lambda: net._run(net._pack(torch.device("cpu")), xin, gold["timesteps"],
-                                                  ctx.reshape(2 * T, -1), y, 2 * T, T, 2, hw, hw, torch.device("cpu")))
+    calls = []
+    with emu_ops.patched(calls):
+        out = net._run(net._pack(torch.device("cpu")), xin, gold["timesteps"], ctx.reshape(2 * T, -1), y, 2 * T, T, 2,
+                       hw, hw, torch.device("cpu"))
     report = [(name, _rel(val[[0, T]][:, ::8], gold["tap:" + name])) for name, val in taps.items()]
     print("duplicated tokens: rel-L2", _rel(out, gold["out"]), "worst tap", max(report, key=lambda t: t[1]))
     assert sum(n == "attention_cross" for n, _, _ in calls) == 32              # 16 transformers x (spatial, temporal)
@@ -256,7 +221,7 @@ def test_multi_token_schedule_reads_the_right_key_sets():
     forward is repeated with one context perturbed at a time.  Changing frame 1's tokens must change frame 1 and leave
     the other samples bit-identical except through the temporal mixing of the same video (frame 1 is not frame 0);
     changing frame 0 of the c half must change every frame of the c half and no frame of the uc half."""
-    import cross_standins
+    import emu_ops
     from oracle import synth
     from v3d_b200.unet import VideoUNet
 
@@ -268,7 +233,7 @@ def test_multi_token_schedule_reads_the_right_key_sets():
     ctx, y = torch.randn(2 * T, M, 1024, generator=g), torch.randn(2 * T, 768, generator=g)
 
     def run(cx):
-        with cross_standins.patched(), torch.no_grad():
+        with emu_ops.patched(), torch.no_grad():
             return net.eval()._run(net._pack(torch.device("cpu")), xin, ts, cx.reshape(2 * T, -1), y, 2 * T, T, 2, hw,
                                    hw, torch.device("cpu"))
 
@@ -329,13 +294,13 @@ def test_sample_views_multi_token_matches_oracle():
     """DiffusionEngine.sample_views with a 3-token context (2 Euler-EDM steps, per-frame CFG, decode) against the oracle
     composition, at the bound smoke() applies."""
     import cpu_shims
-    import cross_standins
+    import emu_ops
     from oracle import ref_decoder, ref_sampling, ref_unet
 
     T, hw, steps = 3, 8, 2
     eng, sd_u, sd_d = cpu_shims.cpu_engine(T, steps)
     x, c, uc = _ctx_cond(T, hw, 3)
-    with cross_standins.patched():
+    with emu_ops.patched():
         frames = eng.sample_views(x.clone(), c, uc, num_frames=T)
     extra = {"image_only_indicator": torch.zeros(2, T), "num_video_frames": T}
     with torch.no_grad():
@@ -359,7 +324,7 @@ def _plan_worker(rank: int, world: int, port: int, T: int, mode: str, q):
     import torch.distributed as dist
 
     import cpu_shims
-    import cross_standins
+    import emu_ops
     from v3d_b200.viewshard import ShardPlan
 
     torch.set_num_threads(2)
@@ -367,7 +332,7 @@ def _plan_worker(rank: int, world: int, port: int, T: int, mode: str, q):
     plan = ShardPlan.create(T, mode)
     eng, _, _ = cpu_shims.cpu_engine(T, 2)
     x, c, uc = _ctx_cond(T, 8, 3)
-    with cross_standins.patched():
+    with emu_ops.patched():
         ref = eng.sample_views(x.clone(), c, uc, num_frames=T)
         mine = eng.sample_views(x.clone(), c, uc, num_frames=T, shard=plan)
         gathered = plan.gather_frames(mine)
@@ -398,14 +363,14 @@ def test_assemble_conditioning_with_k_token_clip_embedding_matches_oracle(k):
     """get_batch + GeneralConditioner + per-frame repeat (V3D_512.py:247-267) with a [1, k, 1024] embedding give
     crossattn [T, k, 1024] (every frame the same k tokens, uc zeros) and the concat latent of the one conditioning
     image, bit for bit as the oracle's conditioning."""
-    import cross_standins
+    import emu_ops
     from oracle import ref_conditioning
     from v3d_b200 import conditioning
 
     T = 5
     g = torch.Generator().manual_seed(43)
     clip_emb, latent = torch.randn(1, k, 1024, generator=g), torch.randn(1, 4, 8, 8, generator=g)
-    with cross_standins.patched():
+    with emu_ops.patched():
         cond = conditioning.GeneralConditioner(conditioning.V3D_512_EMB_MODELS)
         c, uc = conditioning.assemble_v3d_conditioning(cond, clip_emb, latent, 6.0, 127.0, 0.02, T)
     oc, ouc = ref_conditioning.v3d_conditioning(clip_emb, latent, 6.0, 127.0, 0.02, T)

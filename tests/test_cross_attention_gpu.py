@@ -93,7 +93,7 @@ def test_attention_cross_edges(nq, nk, heads):
     zero-filled from TMA and must be masked), key sets packed (kv_bstride = nk) and spaced with NaN rows that must not
     be read, distinct row strides and untouched margins; scores of O(1) and of O(100) nats (the running maximum).  The
     torch stand-in runs on the same operands."""
-    import cross_standins
+    import emu_ops
     from v3d_b200 import ops
 
     nbatch = 1 if nq == 73728 else 2
@@ -103,7 +103,7 @@ def test_attention_cross_edges(nq, nk, heads):
             seed = nq * 7 + nk * 131 + heads * 3 + gap + int(amp)
             q, kv, obuf, bs = _operands(nbatch, nq, nk, heads, gap, amp, seed)
             ref, mag = _reference(q, kv, nbatch, nq, nk, heads, bs)
-            impls = [("kernel", ops.attention_cross)] + ([("standin", cross_standins.attention_cross)] if nq <= 4096 else [])
+            impls = [("kernel", ops.attention_cross)] + ([("standin", emu_ops.attention_cross)] if nq <= 4096 else [])
             for impl, fn in impls:
                 obuf.fill_(SENTINEL)
                 out = obuf[:, 24:24 + c]

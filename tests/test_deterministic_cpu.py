@@ -1,5 +1,5 @@
 """Deterministic mode on the CPU: the C-ABI surface of the deterministic GroupNorm, the mode switch, and the HOST
-SCHEDULES in deterministic mode with the kernels' CPU stand-ins (tests/det_standins.py over tests/emu_ops.py):
+SCHEDULES in deterministic mode with the kernels' CPU stand-ins (tests/emu_ops.py):
 
   * against the oracle, within the usual bf16 parity bound;
   * frame-sharded ('views') and CFG-split ('cfg') plans over gloo against the unsharded deterministic schedule:
@@ -44,11 +44,11 @@ def test_new_entry_points_are_declared_exported_and_bound():
 @pytest.mark.parametrize("rows,hw", [(4096, 4096), (18 * 4096, 4096), (18 * 576, 576), (5 * 64, 64), (3 * 300, 300),
                                      (2 * 262144, 262144), (7, 7)])
 def test_block_geometry_and_workspace_size_match_the_library(rows, hw):
-    import det_standins
+    import emu_ops
     from v3d_b200 import ops
 
-    assert ops.groupnorm_det_blocks(rows, hw) == det_standins.groupnorm_det_blocks(rows, hw)
-    assert ops.groupnorm_det_workspace_bytes(rows, hw, 3) == det_standins.groupnorm_det_workspace_bytes(rows, hw, 3)
+    assert ops.groupnorm_det_blocks(rows, hw) == emu_ops.groupnorm_det_blocks(rows, hw)
+    assert ops.groupnorm_det_workspace_bytes(rows, hw, 3) == emu_ops.groupnorm_det_workspace_bytes(rows, hw, 3)
     r = min(256, hw)
     assert ops.groupnorm_det_blocks(rows, hw) == rows // hw * -(-hw // r)
 
@@ -88,13 +88,13 @@ def test_graph_cache_key_includes_the_mode(monkeypatch):
 
 
 def test_frame_subset_partials_equal_the_whole_tensors():
-    import det_standins
+    import emu_ops
 
     g = torch.Generator().manual_seed(3)
     nb, T, hw, c = 2, 5, 300, 64                                   # blocks of 256 + 44 rows per frame
     x = torch.randn(nb, T, hw, c, generator=g).to(torch.bfloat16)
-    full = det_standins.block_pairs(x.view(-1, c), T * hw, hw, nb, c)
-    sub = det_standins.block_pairs(x[:, 2:4].contiguous().view(-1, c), 2 * hw, hw, nb, c)
+    full = emu_ops.block_pairs(x.view(-1, c), T * hw, hw, nb, c)
+    sub = emu_ops.block_pairs(x[:, 2:4].contiguous().view(-1, c), 2 * hw, hw, nb, c)
     assert full.shape == (nb, T * 2, 32, 2)
     assert torch.equal(sub, full[:, 4:8])
 
@@ -102,52 +102,40 @@ def test_frame_subset_partials_equal_the_whole_tensors():
 def test_det_schedule_selects_the_deterministic_kernels(det_mode):
     """In deterministic mode no norm takes the atomic statistics; the 2-D norms take the single launch, the 3-D norms
     the pair (the same selection as the default mode), and V3D_GN_FUSED=0 moves everything to the pair."""
-    import det_standins
-    from v3d_b200 import ops
+    import emu_ops
 
-    T, hw = 4, 8                                                   # B = 8 samples: the 2-D norms take one launch
+    T, hw = 4, 8                                                  # B = 8 samples: the 2-D norms take one launch
     net, _ = _build_unet()
     xin, ts, ctx, y = _unet_inputs(T, hw)
-    calls = {}
-
-    def counting(name):
-        fn = getattr(ops, name)
-
-        def wrapped(*a, **k):
-            calls[name] = calls.get(name, 0) + 1
-            return fn(*a, **k)
-        return wrapped
-
     names = ["groupnorm_stats", "groupnorm", "groupnorm_det", "groupnorm_partials", "groupnorm_fold_apply"]
-    with det_standins.patched():
-        saved = {n: getattr(ops, n) for n in names}
+
+    def norm_calls(since):
+        return {n: k for n, k in (launches - since).items() if n in names}
+
+    with emu_ops.patched() as launches:
+        n0 = launches.copy()
+        P = net._pack(torch.device("cpu"))
+        _run_unet(net, P, xin, ts, ctx.reshape(2 * T, -1), y, T)
+        first = norm_calls(n0)
+        n1 = launches.copy()
+        os.environ["V3D_GN_FUSED"] = "0"
         try:
-            for n in names:
-                setattr(ops, n, counting(n))
-            P = net._pack(torch.device("cpu"))
             _run_unet(net, P, xin, ts, ctx.reshape(2 * T, -1), y, T)
-            first = dict(calls)
-            calls.clear()
-            os.environ["V3D_GN_FUSED"] = "0"
-            try:
-                _run_unet(net, P, xin, ts, ctx.reshape(2 * T, -1), y, T)
-            finally:
-                del os.environ["V3D_GN_FUSED"]
         finally:
-            for n, f in saved.items():
-                setattr(ops, n, f)
+            del os.environ["V3D_GN_FUSED"]
+        calls = norm_calls(n1)
     assert first == {"groupnorm_det": 61, "groupnorm_partials": 44, "groupnorm_fold_apply": 44}, first
     assert calls == {"groupnorm_partials": 105, "groupnorm_fold_apply": 105}, calls
 
 
 def test_det_unet_and_decoder_schedules_match_oracle(det_mode):
-    import det_standins
+    import emu_ops
     from oracle import ref_decoder, ref_unet
 
     T, hw = 3, 16
     net, sd = _build_unet()
     xin, ts, ctx, y = _unet_inputs(T, hw)
-    with det_standins.patched():
+    with emu_ops.patched():
         out = _run_unet(net, net._pack(torch.device("cpu")), xin, ts, ctx.reshape(2 * T, -1), y, T)
     with torch.no_grad():
         ref = ref_unet.unet_forward(sd, ref_unet.UNetSpec(model_channels=64), xin, ts, ctx, y, T, torch.zeros(2, T))
@@ -157,7 +145,7 @@ def test_det_unet_and_decoder_schedules_match_oracle(det_mode):
 
     dec, sdd = _build_decoder()
     z = torch.randn(T, 4, 8, 8, generator=torch.Generator().manual_seed(3))
-    with det_standins.patched(), torch.no_grad():
+    with emu_ops.patched(), torch.no_grad():
         out = dec._run(dec._pack(torch.device("cpu")), z, T, T, 1, 8, 8)
         ref = ref_decoder.decoder_forward(sdd, ref_decoder.DecoderSpec(ch=64), z, T)
     r, cs = _rel(out, ref), _cos(out, ref)
@@ -175,7 +163,7 @@ def _views_worker(rank: int, world: int, port: int, T: int, q):
                       MASTER_PORT=str(port), V3D_DETERMINISTIC="1")
     import torch.distributed as dist
 
-    import det_standins
+    import emu_ops
     from v3d_b200.viewshard import ViewShard
 
     torch.set_num_threads(2)
@@ -183,7 +171,7 @@ def _views_worker(rank: int, world: int, port: int, T: int, q):
     vs = ViewShard.create(T)
     res = {"rank": rank, "block": (vs.t0, vs.tl)}
     pick = torch.cat([torch.arange(vs.t0, vs.t0 + vs.tl), T + torch.arange(vs.t0, vs.t0 + vs.tl)])
-    with det_standins.patched(), torch.no_grad():
+    with emu_ops.patched(), torch.no_grad():
         net, _ = _build_unet()
         P = net._pack(torch.device("cpu"))
         xin, ts, ctx, y = _unet_inputs(T, 16)
@@ -234,7 +222,7 @@ def _plan_worker(rank: int, world: int, port: int, T: int, mode: str, q):
     import torch.distributed as dist
 
     import cpu_shims
-    import det_standins
+    import emu_ops
     from oracle import synth
     from v3d_b200.viewshard import ShardPlan
 
@@ -245,7 +233,7 @@ def _plan_worker(rank: int, world: int, port: int, T: int, mode: str, q):
     x, c, uc = synth.synth_inputs(T, 8)
     g = torch.Generator().manual_seed(5)
     c = dict(c, crossattn=c["crossattn"] + 0.5 * torch.randn(T, 1, 1024, generator=g))
-    with det_standins.patched():
+    with emu_ops.patched():
         ref = eng.sample_views(x.clone(), c, uc, num_frames=T)
         mine = eng.sample_views(x.clone(), c, uc, num_frames=T, shard=plan)
         gathered = plan.gather_frames(mine)

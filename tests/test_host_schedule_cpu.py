@@ -315,7 +315,7 @@ def test_sampler_variants_host_path_match_reference_golden(tag):
               "central": {"target": base + "guiders.CentralPredictionGuider",
                           "params": {"max_scale": m["max_scale"], "min_scale": m["min_scale"], "num_frames": T}},
               "vanilla": {"target": base + "guiders.VanillaCFG", "params": {"scale": m.get("vanilla_scale", 2.5)}}}[kind]
-    shim = {"EulerEDMSampler": cpu_shims.CpuEuler, "HeunEDMSampler": cpu_shims.CpuHeun}[m.get("sampler", "EulerEDMSampler")]
+    shim = cpu_shims.CPU_SHIMS[m.get("sampler", "EulerEDMSampler")]
     sampler = shim(num_steps=m["num_steps"],
                    discretization_config={"target": base + "discretizer.EDMDiscretization",
                                           "params": {"sigma_max": m["sigma_max"]}}, guider_config=guider)
@@ -363,7 +363,7 @@ def test_sampler_variants_logic_exact_with_fp32_network(tag):
               "central": {"target": base + "guiders.CentralPredictionGuider",
                           "params": {"max_scale": m["max_scale"], "min_scale": m["min_scale"], "num_frames": T}},
               "vanilla": {"target": base + "guiders.VanillaCFG", "params": {"scale": m.get("vanilla_scale", 2.5)}}}[kind]
-    shim = {"EulerEDMSampler": cpu_shims.CpuEuler, "HeunEDMSampler": cpu_shims.CpuHeun}[m.get("sampler", "EulerEDMSampler")]
+    shim = cpu_shims.CPU_SHIMS[m.get("sampler", "EulerEDMSampler")]
     sampler = shim(num_steps=m["num_steps"],
                    discretization_config={"target": base + "discretizer.EDMDiscretization",
                                           "params": {"sigma_max": m["sigma_max"]}}, guider_config=guider)
@@ -431,7 +431,7 @@ def _plan_worker(rank: int, world: int, port: int, T: int, mode: str, q, sampler
     torch.set_num_threads(2)
     dist.init_process_group("gloo", rank=rank, world_size=world)
     plan = ShardPlan.create(T, mode)
-    eng, _, _ = cpu_shims.cpu_engine(T, 2, sampler_cls=cpu_shims.CpuHeun if sampler == "heun" else cpu_shims.CpuEuler)
+    eng, _, _ = cpu_shims.cpu_engine(T, 2, sampler="HeunEDMSampler" if sampler == "heun" else "EulerEDMSampler")
     x, c, uc = synth.synth_inputs(T, 8)
     g = torch.Generator().manual_seed(5)
     c = dict(c, crossattn=c["crossattn"] + 0.5 * torch.randn(T, 1, 1024, generator=g))

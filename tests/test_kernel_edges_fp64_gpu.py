@@ -51,7 +51,7 @@ rows at rows 0, rows-1 and 2^k +- 1, a constant group, a group with variance ~ e
 64 (how far the one-pass fp32 (sum x, sum x^2) holds).
 
 Every case runs over `impl`: the kernel on CUDA (marked gpu), and, where one exists, the CPU stand-in of
-tests/emu_ops.py / tests/det_standins.py on a reduced shape list (unmarked), which runs the builders, the oracle and
+tests/emu_ops.py on a reduced shape list (unmarked), which runs the builders, the oracle and
 the index decoding without a GPU and pins the stand-ins at the same edges.
 
 Each check prints one `EDGE <family> <case> ratio=<max |err| / bound> exact=<rate>` line (visible with -s or -rA).
@@ -66,7 +66,6 @@ import torch.nn.functional as F
 
 sys.path.insert(0, str(Path(__file__).resolve().parent))
 
-import det_standins  # noqa: E402
 import emu_ops  # noqa: E402
 from v3d_b200 import ops  # noqa: E402
 
@@ -751,7 +750,7 @@ def test_groupnorm_edges(variant, C, ns, frames, hw, silu, impl):
     mag = back(core) * gamma.abs() + beta.abs()
     if silu:
         y = y * torch.sigmoid(y)
-    o = ops if impl == "kernel" else (det_standins if variant.startswith("det") else emu_ops)
+    o = ops if impl == "kernel" else emu_ops
     xd, gd, bd = _bf(x.reshape(ns * rows, C), dev), gamma.float().to(dev), beta.float().to(dev)
     out = Guarded(ns * rows, C, BF, dev)
     if variant == "pair":

@@ -1,7 +1,6 @@
-"""Videos of more than 32 view-frames (up to 128), on CPU with the kernels' stand-ins (tests/emu_ops.py,
-tests/cross_standins.py, and tests/longt_standins.py for the two temporal attention entry points):
+"""Videos of more than 32 view-frames (up to 128), on CPU with the kernels' stand-ins (tests/emu_ops.py):
 
-  * the stand-ins of tests/longt_standins.py against an fp64 softmax attention written out per sequence, dense and
+  * the temporal attention stand-ins against an fp64 softmax attention written out per sequence, dense and
     through a shuffled, padded, rank-major row table;
   * the UNet schedule and a 3-step Euler-EDM trajectory against fixtures of the REAL reference at T = 40 and T = 48
     (tests/golden/unet_small_t40.pt, unet_full_t48_16.pt, edm_small_t40.pt), at the bounds of the T <= 32 fixtures;
@@ -90,7 +89,7 @@ def sequence_reference(qkv, nb, T, s, heads, scale):
                                            (48, [(0, 12), (12, 12), (24, 12), (36, 12)], 3),
                                            (128, [(0, 16)] + [(16 * i, 16) for i in range(1, 8)], 5)])
 def test_temporal_standins_match_fp64(T, blocks, rank):
-    import longt_standins
+    import emu_ops
 
     nb, s, heads = 2, 3, 2
     c = heads * 64
@@ -98,7 +97,7 @@ def test_temporal_standins_match_fp64(T, blocks, rank):
     qkv = (torch.randn(nb * T * s, 3 * c, generator=g) * 2.0).to(torch.bfloat16)
     ref = sequence_reference(qkv, nb, T, s, heads, 0.125)
     dense = torch.zeros(nb * T * s, c, dtype=torch.bfloat16)
-    longt_standins.attention_temporal(qkv, dense, nb, T, s, heads, 0.125)
+    emu_ops.attention_temporal(qkv, dense, nb, T, s, heads, 0.125)
     assert ((dense.double() - ref).abs() <= 2.0 ** -8 * ref.abs()).all()                    # fp64, one bf16 rounding
     order = list(range(len(blocks)))[::-1]
     row, bstride, nrows = shuffled_table(blocks, nb, s, order)
@@ -106,7 +105,7 @@ def test_temporal_standins_match_fp64(T, blocks, rank):
     t0, tl = blocks[rank]
     ql = qkv.view(nb, T, s, 3 * c)[:, t0:t0 + tl].reshape(nb * tl * s, 3 * c)
     out = torch.zeros(nb * tl * s, c, dtype=torch.bfloat16)
-    longt_standins.attention_temporal_kv(ql, buf, out, nb, tl, s, heads, row, bstride, 0.125)
+    emu_ops.attention_temporal_kv(ql, buf, out, nb, tl, s, heads, row, bstride, 0.125)
     assert torch.equal(out, dense.view(nb, T, s, c)[:, t0:t0 + tl].reshape(nb * tl * s, c))
 
 
@@ -131,7 +130,6 @@ def test_unet_long_video_schedule_matches_reference_golden(tag):
     """Output rel-L2 3e-2 / cosine 0.999 for the whole tensor and every sample, block taps 2e-2: the bounds of the
     T <= 32 fixtures."""
     import emu_ops
-    import longt_standins
     from make_golden_longt import unet_inputs
 
     m = _manifest(tag)
@@ -143,7 +141,7 @@ def test_unet_long_video_schedule_matches_reference_golden(tag):
     taps = {k[4:]: None for k in gold if k.startswith("tap:")}
     net.debug_taps = taps
     B, _, H, W = xin.shape
-    with longt_standins.patched(), torch.no_grad():
+    with emu_ops.patched(), torch.no_grad():
         n0 = emu_ops.launch_count()
         out = net._run(net._pack(torch.device("cpu")), xin, ts, ctx.reshape(B, -1), y, B, T, B // T, H, W,
                        torch.device("cpu"))
@@ -160,7 +158,7 @@ def test_unet_long_video_schedule_matches_reference_golden(tag):
 def test_edm_long_video_trajectory_matches_reference_golden():
     """3 Euler-EDM steps under LinearPredictionGuider(num_frames=40) through the drop-in sampler / denoiser / wrapper."""
     import cpu_shims
-    import longt_standins
+    import emu_ops
     from oracle import synth
     from v3d_b200 import sampling
 
@@ -179,7 +177,7 @@ def test_edm_long_video_trajectory_matches_reference_golden():
     den = sampling.Denoiser({"target": "v3d_b200.sgm.modules.diffusionmodules.denoiser_scaling.VScalingWithEDMcNoise"})
     model = sampling.OpenAIWrapper(net)
     extra = {"image_only_indicator": torch.zeros(2, T), "num_video_frames": T}
-    with longt_standins.patched():
+    with emu_ops.patched():
         out = sampler(lambda i, s, cc: den(model, i, s, cc, **extra), x.clone(), cond=c, uc=uc)
     r = _rel(out, gold["out"])
     print("edm_small_t40 rel-L2", r)
@@ -212,7 +210,7 @@ def _plan_worker(rank: int, world: int, port: int, T: int, mode: str, q):
     import torch.distributed as dist
 
     import cpu_shims
-    import longt_standins
+    import emu_ops
     from oracle import synth
     from v3d_b200.viewshard import ShardPlan
 
@@ -221,7 +219,7 @@ def _plan_worker(rank: int, world: int, port: int, T: int, mode: str, q):
     plan = ShardPlan.create(T, mode)
     eng, _, _ = cpu_shims.cpu_engine(T, 1)
     x, c, uc = synth.synth_inputs(T, 8)
-    with longt_standins.patched():
+    with emu_ops.patched():
         ref = eng.sample_views(x.clone(), c, uc, num_frames=T, decoding_t=T)    # a sharded video decodes as one chunk
         mine = eng.sample_views(x.clone(), c, uc, num_frames=T, shard=plan)
         gathered = plan.gather_frames(mine)
@@ -252,7 +250,6 @@ def test_sharded_plans_match_unsharded_long_video_gloo(mode, world, T):
 def test_more_than_128_frames_is_refused_before_any_launch():
     import cpu_shims
     import emu_ops
-    import longt_standins
     from v3d_b200 import ops
     from v3d_b200.unet import VideoUNet
     from v3d_b200.viewshard import ViewShard
@@ -266,7 +263,7 @@ def test_more_than_128_frames_is_refused_before_any_launch():
         xin, ts, y = torch.zeros(2 * T, 8, 8, 8), torch.zeros(2 * T), torch.zeros(2 * T, 768)
         return net(xin, ts, torch.zeros(2 * T, 1, 1024), y, tc, T, torch.zeros(2, T))
 
-    with longt_standins.patched():
+    with emu_ops.patched():
         n0 = emu_ops.launch_count()
         with pytest.raises(ValueError, match="temporal attention supports at most 128 frames, got 129"):
             call(129)
@@ -295,22 +292,10 @@ def test_front_end_takes_48_frames():
 # ---------------------------------------------------------------------------------------------------------------
 # T <= 32 is untouched
 # ---------------------------------------------------------------------------------------------------------------
-def _describe(v):
-    if isinstance(v, torch.Tensor):
-        return ("T", tuple(v.shape), str(v.dtype), tuple(v.stride()))
-    if isinstance(v, (list, tuple)):
-        return tuple(_describe(e) for e in v)
-    if isinstance(v, float):
-        return round(v, 9)
-    return v
-
-
 def short_forward_calls(T, hw=8):
-    """Every ops call ([(name, args, kwargs)], tensors as shapes) of one forward of the width-64 UNet."""
-    import cross_standins
-    import longt_standins
+    """Every ops launch ([(name, args, kwargs)], tensors as shapes) of one forward of the width-64 UNet."""
+    import emu_ops
     from oracle import synth
-    from v3d_b200 import ops
     from v3d_b200.unet import VideoUNet
 
     net = VideoUNet(**UNET_KW)
@@ -321,26 +306,9 @@ def short_forward_calls(T, hw=8):
     y = torch.cat([uc["vector"], c["vector"]])
     ts = torch.linspace(-0.5, 1.2, 2 * T)
     calls = []
-    with longt_standins.patched():
-        saved = {}
-        for n in cross_standins.EMULATED:
-            if n in ("launch_count", "groupnorm_workspace"):
-                continue
-            f = getattr(ops, n)
-            saved[n] = f
-
-            def rec(*a, _n=n, _f=f, **kw):
-                calls.append((_n, _describe(a), tuple(sorted((k, _describe(v)) for k, v in kw.items()))))
-                return _f(*a, **kw)
-
-            setattr(ops, n, rec)
-        try:
-            with torch.no_grad():
-                net._run(net._pack(torch.device("cpu")), xin, ts, ctx.reshape(2 * T, -1), y, 2 * T, T, 2, hw, hw,
-                         torch.device("cpu"))
-        finally:
-            for n, f in saved.items():
-                setattr(ops, n, f)
+    with emu_ops.patched(calls), torch.no_grad():
+        net._run(net._pack(torch.device("cpu")), xin, ts, ctx.reshape(2 * T, -1), y, 2 * T, T, 2, hw, hw,
+                 torch.device("cpu"))
     return calls
 
 

@@ -1,6 +1,6 @@
 """Videos of more than 32 view-frames on the H100: attn_temporal_long_kernel (33 <= T <= 128) in fp64 at its tile
 edges, its frame-sharded form against the dense one bit for bit, which kernel each T launches, the stand-ins of
-tests/longt_standins.py against the kernel, and the native UNet / sampler / engine at T = 40 and T = 48 against the
+tests/emu_ops.py against the kernel, and the native UNet / sampler / engine at T = 40 and T = 48 against the
 real reference's fixtures, under CUDA graphs, in deterministic mode and frame-sharded over the peer transport.  The
 CPU twins are in tests/test_long_video_cpu.py."""
 import json
@@ -95,14 +95,14 @@ def test_attention_temporal_long_edges(T, S, heads, nb):
     tile, both key capacities (64 / 128), row strides wider than 3C / C with NaN padding that must not be read and
     sentinel margins and tail rows that must not be written; the other video's rows turned to NaN must not change this
     video's output.  The torch stand-in runs on the same operands where they are small."""
-    import longt_standins
+    import emu_ops
     from v3d_b200 import ops
 
     c = heads * 64
     rows = nb * T * S
     qkv = _qkv(nb, T, S, heads, seed=T * 131 + S + heads)
     ref, mag = _reference(qkv, nb, T, S, heads)
-    impls = [("kernel", ops.attention_temporal)] + ([("standin", longt_standins.attention_temporal)] if S <= 64 else [])
+    impls = [("kernel", ops.attention_temporal)] + ([("standin", emu_ops.attention_temporal)] if S <= 64 else [])
     for impl, fn in impls:
         obuf = torch.full((rows + 8, c + 16), SENTINEL, device=DEV, dtype=BF)
         fn(qkv, obuf, nb, T, S, heads, SCALE)
@@ -156,10 +156,10 @@ def test_split_kv_equals_dense_bit_for_bit(tq, tk, blocks, rank, S, heads):
     ref, mag = _reference(qkv, nb, tk, S, heads, f0, tq)
     _check(f"split Tq={tq} Tk={tk} S={S} heads={heads}", obuf[:, :c], ref, mag)
     if S == 64:
-        import longt_standins
+        import emu_ops
 
         sbuf = torch.full_like(obuf, SENTINEL)
-        longt_standins.attention_temporal_kv(ql, buf, sbuf, nb, tq, S, heads, row, bstride, SCALE)
+        emu_ops.attention_temporal_kv(ql, buf, sbuf, nb, tq, S, heads, row, bstride, SCALE)
         _check(f"split standin Tq={tq} Tk={tk}", sbuf[:, :c], ref, mag, 0.0)
         assert (sbuf[:, c:] == SENTINEL).all()
 

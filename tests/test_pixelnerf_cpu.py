@@ -1,5 +1,5 @@
 """PixelNeRF scene conditioning without a GPU: the oracle against the reference fixtures, the state_dict layout, and
-the host logic of PixelNeRF / PixelNeRFEmbedder / ExtraConditioner through the stand-ins of tests/pixelnerf_standins.py
+the host logic of PixelNeRF / PixelNeRFEmbedder / ExtraConditioner through the stand-ins of tests/emu_ops.py
 (key order, the `rgb` key, the uc zeros, the "(b t)" repeat, and the jitter draws of the c and uc passes)."""
 from __future__ import annotations
 
@@ -11,7 +11,7 @@ import torch
 
 sys.path.insert(0, str(Path(__file__).resolve().parent))
 
-import pixelnerf_standins  # noqa: E402
+import emu_ops  # noqa: E402
 from oracle import ref_pixelnerf as R  # noqa: E402
 
 GOLDEN = Path(__file__).parent / "golden"
@@ -68,8 +68,10 @@ def test_module_through_standins_meets_fixture(tag):
 
     emb = _embedder(cs, sampler)
     emb.pixelnerf_encoder.load_state_dict(fx["state_dict"])
-    with pixelnerf_standins.patched() as calls:
+    with emu_ops.patched() as launches:
+        n0 = launches.copy()
         rgb, fe = emb(fx["inputs"])
+    calls = launches - n0
     assert dict(calls) == {"pixelnerf_rays": 1, "pixelnerf_render": 1, "pixelnerf_decode": 1}
     assert shapes == [(cs["ns"], cs["B"] * cs["T"], cs["render_size"] ** 2, 1)]
     assert rgb.shape == fx["rgb"].shape and fe.shape == fx["feats"].shape
@@ -120,8 +122,10 @@ def test_extra_conditioner_meets_reference(tag="scene_s1"):
     cond.embedders[1].pixelnerf_encoder.load_state_dict(fx["state_dict"])
     batch = dict(ref["batch"], pixelnerf_input=fx["inputs"])
     keys = ["cond_frames", "pixelnerf_input", "clip"]
-    with pixelnerf_standins.patched() as calls:
+    with emu_ops.patched() as launches:
+        n0 = launches.copy()
         c, uc = cond.get_unconditional_conditioning(batch, force_uc_zero_embeddings=keys)
+    calls = launches - n0
     # the embedder runs for c and for uc, and draws its jitter both times, in the reference's shape
     assert calls["pixelnerf_render"] == 2 and draws == [(cs["ns"], B * T, rs * rs, 1)] * 2
     assert list(c.keys()) == ref["c_keys"] == ["concat", "rgb", "crossattn"] and list(uc.keys()) == ref["uc_keys"]

@@ -1,7 +1,7 @@
 """EulerAncestralSampler, DPMPP2SAncestralSampler, DPMPP2MSampler and LinearMultistepSampler without a GPU: the oracle
 against the real reference's outputs (tests/golden/edm_small_{euler_ancestral,dpmpp2s,dpmpp2m,lms}.pt, written by
 oracle/make_golden_samplers.py), the drop-in classes' host logic with their step kernels' torch stand-ins
-(tests/sampler_standins.py), and the sharded plans of DiffusionEngine.sample_views over gloo.
+(tests/emu_ops.py), and the sharded plans of DiffusionEngine.sample_views over gloo.
 """
 import json
 import os
@@ -89,7 +89,8 @@ def test_dropin_logic_exact_with_fp32_network(tag):
     """The drop-in samplers (step kernels as stand-ins) around the ORACLE's fp32 UNet reproduce the real reference's
     outputs to fp32 rounding: schedule, multipliers, skipped evaluations, history and the injected noise, in order.
     They also evaluate the network exactly as often as the reference did."""
-    import sampler_standins as ss
+    import cpu_shims
+    import emu_ops
     from oracle import make_golden_samplers as mgs
     from oracle import ref_unet, synth
     from v3d_b200 import sampling
@@ -100,7 +101,7 @@ def test_dropin_logic_exact_with_fp32_network(tag):
     sd = synth.synth_state_dict(ref_unet.unet_param_shapes(spec), seed=mu["weight_seed"])
     T, hw = m["T"], m["latent_hw"]
     x, c, uc = synth.synth_inputs(T, hw)
-    sampler = _dropin(ss.CPU_SHIMS[m["sampler"]], m, T)
+    sampler = _dropin(cpu_shims.CPU_SHIMS[m["sampler"]], m, T)
     if m.get("noise_seed") is not None:
         sampler.noise_sampler = mgs.seeded_noise(m["noise_seed"])
     den = sampling.Denoiser({"target": BASE + "denoiser_scaling.VScalingWithEDMcNoise"})
@@ -112,7 +113,7 @@ def test_dropin_logic_exact_with_fp32_network(tag):
 
     extra = {"image_only_indicator": torch.zeros(2, T), "num_video_frames": T}
     evals = [0]
-    with ss.patched():
+    with emu_ops.patched():
         out = sampler(_counting(lambda i, s, cc: den(OracleNet(), i, s, cc, **extra), evals), x.clone(), cond=c, uc=uc)
     r = _rel(out, gold["out"])
     print(tag, "sampler logic with fp32 network vs reference golden: rel-L2", r, "evals", evals[0])
@@ -125,7 +126,7 @@ def test_dropin_host_path_with_bf16_unet_matches_reference_golden(tag):
     """The drop-in samplers through the drop-in Denoiser / OpenAIWrapper / VideoUNet host schedule with every kernel
     as its CPU stand-in (bf16 network), against the real reference's fp32 outputs: the GPU parity bound, rel-L2 3e-2."""
     import cpu_shims
-    import sampler_standins as ss
+    import emu_ops
     from oracle import make_golden_samplers as mgs
     from oracle import synth
     from v3d_b200 import sampling
@@ -138,14 +139,14 @@ def test_dropin_host_path_with_bf16_unet_matches_reference_golden(tag):
     net.__class__ = cpu_shims.CpuUNet
     T, hw = m["T"], m["latent_hw"]
     x, c, uc = synth.synth_inputs(T, hw)
-    sampler = _dropin(ss.CPU_SHIMS[m["sampler"]], m, T)
+    sampler = _dropin(cpu_shims.CPU_SHIMS[m["sampler"]], m, T)
     if m.get("noise_seed") is not None:
         sampler.noise_sampler = mgs.seeded_noise(m["noise_seed"])
     den = sampling.Denoiser({"target": BASE + "denoiser_scaling.VScalingWithEDMcNoise"})
     model = sampling.OpenAIWrapper(net.eval())
     extra = {"image_only_indicator": torch.zeros(2, T), "num_video_frames": T}
     x0 = x.clone()
-    with ss.patched():
+    with emu_ops.patched():
         out = sampler(lambda i, s, cc: den(model, i, s, cc, **extra), x0, cond=c, uc=uc)
     r = _rel(out, gold["out"])
     print(tag, "host path vs reference golden: rel-L2", r)
@@ -173,12 +174,14 @@ def test_noise_calls_and_network_evaluations(name):
     network runs N times for N steps (DPM++ 2S: 2N - 1, the last step has no midpoint).  sigma_max 80 keeps every
     sigma_down of this schedule nonzero in fp32 (a step from 700 straight down to 0.002 rounds it to exactly 0, and the
     reference then skips that midpoint too)."""
-    import sampler_standins as ss
+    import cpu_shims
+    import emu_ops
 
     T, hw, steps = 3, 4, 4
-    sampler = ss.CPU_SHIMS[name](num_steps=steps, discretization_config={"target": BASE + "discretizer.EDMDiscretization"},
-                                 guider_config={"target": BASE + "guiders.LinearPredictionGuider",
-                                                "params": {"max_scale": 2.5, "num_frames": T}})
+    sampler = cpu_shims.CPU_SHIMS[name](num_steps=steps,
+                                        discretization_config={"target": BASE + "discretizer.EDMDiscretization"},
+                                        guider_config={"target": BASE + "guiders.LinearPredictionGuider",
+                                                       "params": {"max_scale": 2.5, "num_frames": T}})
     calls = []
     if hasattr(sampler, "noise_sampler"):
         default = sampler.noise_sampler
@@ -187,7 +190,7 @@ def test_noise_calls_and_network_evaluations(name):
     g = torch.Generator().manual_seed(0)
     x = torch.randn(T, 4, hw, hw, generator=g)
     c = {"crossattn": torch.randn(T, 1, 8, generator=g), "vector": torch.randn(T, 8, generator=g)}
-    with ss.patched():
+    with emu_ops.patched():
         out = sampler(_counting(lambda i, s, cc: 0.5 * i, n_eval), x, cond=c, uc={k: 0 * v for k, v in c.items()})
     assert torch.isfinite(out).all()
     assert n_eval[0] == EVALS_PER_STEPS[name](steps), (name, n_eval[0])
@@ -306,7 +309,8 @@ def _plan_worker(rank: int, world: int, port: int, T: int, mode: str, q):
                       MASTER_PORT=str(port))
     import torch.distributed as dist
 
-    import sampler_standins as ss
+    import cpu_shims
+    import emu_ops
     from oracle import synth
     from v3d_b200.viewshard import ShardPlan
 
@@ -318,9 +322,9 @@ def _plan_worker(rank: int, world: int, port: int, T: int, mode: str, q):
     c = dict(c, crossattn=c["crossattn"] + 0.5 * torch.randn(T, 1, 1024, generator=g))
     res = {"rank": rank, "decode_block": (plan.decode.t0, plan.decode.tl), "cases": {}}
     for name, steps in PLAN_SAMPLERS:
-        eng, _, _ = ss.cpu_engine(name, T, steps)
+        eng, _, _ = cpu_shims.cpu_engine(T, steps, sampler=name)
         gathers = plan.cfg.exchanges if plan.cfg is not None else 0
-        with ss.patched():
+        with emu_ops.patched():
             torch.manual_seed(1234)                     # every rank (and the unsharded call) seeds identically
             ref = eng.sample_views(x.clone(), c, uc, num_frames=T)
             torch.manual_seed(1234)

@@ -1,7 +1,7 @@
 """The ancestral / DPM++ / LMS step kernels and their drop-in samplers on the GPU.
 
   * kernels against an fp64 restatement of their formulas (rel-L2 <= 1e-6: fp32 rounding) and bit for bit against
-    their torch stand-ins (tests/sampler_standins.py, same operation order), at the V3D_512 state size and at an odd
+    their torch stand-ins (tests/emu_ops.py, same operation order), at the V3D_512 state size and at an odd
     per-sample size, with sigma_next = 0 rows and `out` aliasing `x`;
   * the four drop-ins with the bf16 VideoUNet (unet_small weights) and the fixtures' seeded noise against the real
     reference's outputs (tests/golden/edm_small_{euler_ancestral,dpmpp2s,dpmpp2m,lms}.pt);
@@ -41,11 +41,11 @@ def _rel(a, b):
 def _run_both(name, make_args, alias: bool):
     """Kernel and stand-in on identical inputs; `make_args(out)` builds the argument list around the output buffer
     (alias: out is x itself).  Returns (kernel result, stand-in result, the kernel's arguments)."""
-    import sampler_standins as ss
+    import emu_ops
     from v3d_b200 import ops
 
     results = []
-    for impl in (ops, ss):
+    for impl in (ops, emu_ops):
         args = make_args(None if alias else "fresh")
         getattr(impl, name)(*args)
         results.append(args)

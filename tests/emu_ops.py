@@ -19,6 +19,7 @@ kernels on the same CUDA tensors.
 from __future__ import annotations
 
 import contextlib
+import hashlib
 import math
 from collections import Counter
 
@@ -49,6 +50,19 @@ def launch_count() -> int:
 
 pick_block_n = real_ops.pick_block_n      # host functions of the library (no GPU involved)
 geglu_perm = real_ops.geglu_perm
+_require_cuda_current_device = real_ops.require_current_device
+
+
+def require_current_device(t, who):
+    """The entry points' CUDA gate with CPU tensors let through, so that `patched()` alone runs any module, sampler or
+    engine on CPU; a CUDA tensor gets the real check."""
+    if t.is_cuda:
+        _require_cuda_current_device(t, who)
+
+
+def digest(record: list) -> tuple:
+    """(launches, sha256) of a launch record of `patched(record)`: pins a whole schedule's kernels, arguments and order."""
+    return len(record), hashlib.sha256(repr(record).encode()).hexdigest()
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -572,9 +586,10 @@ ENTRY_POINTS = ["launch_count", "gemm", "groupnorm_stats", "groupnorm_apply", "g
                 "copy_channels", "im2col3x3", "nchw_f32_to_nhwc_bf16", "nhwc_to_nchw_f32", "small_linear",
                 "timestep_embedding", "time_mix_conv", "edm_scale_input", "edm_denoise_combine", "cfg_combine",
                 "euler_step", "heun_step", "ancestral_euler_step", "dpmpp2s_stage", "dpmpp2s_step", "dpmpp2m_step",
-                "lms_step", "frames_nchw_to_u8", "pixelnerf_rays", "pixelnerf_render", "pixelnerf_decode"]
+                "lms_step", "frames_nchw_to_u8", "pixelnerf_rays", "pixelnerf_render", "pixelnerf_decode",
+                "require_current_device"]
 HOST_HELPERS = {"launch_count", "groupnorm_workspace", "groupnorm_det_blocks", "groupnorm_det_workspace_bytes",
-                "groupnorm_det_workspace"}
+                "groupnorm_det_workspace", "require_current_device"}
 
 
 def _describe(v):

@@ -16,7 +16,7 @@ import torch
 ROOT = str(Path(__file__).resolve().parent.parent)
 sys.path.insert(0, str(Path(__file__).resolve().parent))
 
-from test_host_schedule_cpu import _build_decoder, _build_unet, _cos, _rel, _run_unet, _unet_inputs  # noqa: E402
+from test_host_schedule_cpu import _build_decoder, _build_unet, _cos, _rel, _unet, _unet_inputs  # noqa: E402
 
 NEW_SYMBOLS = ["v3d_groupnorm_det_blocks", "v3d_groupnorm_det_workspace_bytes", "v3d_groupnorm_partials",
                "v3d_groupnorm_fold_apply", "v3d_groupnorm_det"]
@@ -114,13 +114,12 @@ def test_det_schedule_selects_the_deterministic_kernels(det_mode):
 
     with emu_ops.patched() as launches:
         n0 = launches.copy()
-        P = net._pack(torch.device("cpu"))
-        _run_unet(net, P, xin, ts, ctx.reshape(2 * T, -1), y, T)
+        _unet(net, xin, ts, ctx, y, T)
         first = norm_calls(n0)
         n1 = launches.copy()
         os.environ["V3D_GN_FUSED"] = "0"
         try:
-            _run_unet(net, P, xin, ts, ctx.reshape(2 * T, -1), y, T)
+            _unet(net, xin, ts, ctx, y, T)
         finally:
             del os.environ["V3D_GN_FUSED"]
         calls = norm_calls(n1)
@@ -136,7 +135,7 @@ def test_det_unet_and_decoder_schedules_match_oracle(det_mode):
     net, sd = _build_unet()
     xin, ts, ctx, y = _unet_inputs(T, hw)
     with emu_ops.patched():
-        out = _run_unet(net, net._pack(torch.device("cpu")), xin, ts, ctx.reshape(2 * T, -1), y, T)
+        out = _unet(net, xin, ts, ctx, y, T)
     with torch.no_grad():
         ref = ref_unet.unet_forward(sd, ref_unet.UNetSpec(model_channels=64), xin, ts, ctx, y, T, torch.zeros(2, T))
     r, cs = _rel(out, ref), _cos(out, ref)
@@ -145,8 +144,9 @@ def test_det_unet_and_decoder_schedules_match_oracle(det_mode):
 
     dec, sdd = _build_decoder()
     z = torch.randn(T, 4, 8, 8, generator=torch.Generator().manual_seed(3))
-    with emu_ops.patched(), torch.no_grad():
-        out = dec._run(dec._pack(torch.device("cpu")), z, T, T, 1, 8, 8)
+    with emu_ops.patched():
+        out = dec(z, timesteps=T)
+    with torch.no_grad():
         ref = ref_decoder.decoder_forward(sdd, ref_decoder.DecoderSpec(ch=64), z, T)
     r, cs = _rel(out, ref), _cos(out, ref)
     print("det decoder schedule vs oracle: rel-L2", r, "cos", cs)
@@ -171,28 +171,26 @@ def _views_worker(rank: int, world: int, port: int, T: int, q):
     vs = ViewShard.create(T)
     res = {"rank": rank, "block": (vs.t0, vs.tl)}
     pick = torch.cat([torch.arange(vs.t0, vs.t0 + vs.tl), T + torch.arange(vs.t0, vs.t0 + vs.tl)])
-    with emu_ops.patched(), torch.no_grad():
+    with emu_ops.patched():
         net, _ = _build_unet()
-        P = net._pack(torch.device("cpu"))
         xin, ts, ctx, y = _unet_inputs(T, 16)
-        full = _run_unet(net, P, xin, ts, ctx.reshape(2 * T, -1), y, T)
+        full = _unet(net, xin, ts, ctx, y, T)
         tc = torch.stack([ctx[0], ctx[T]])
         net.view_shard = vs
         try:
-            args, dims, _ = net._prepare(xin[pick], ts[pick], ctx[pick], y[pick], tc, vs.tl, torch.zeros(2, vs.tl))
-            part = net._run(P, *args, *dims, torch.device("cpu"))
+            part = net(xin[pick], ts[pick], ctx[pick], y[pick], time_context=tc, num_video_frames=vs.tl,
+                       image_only_indicator=torch.zeros(2, vs.tl))
         finally:
             net.view_shard = None
         res["unet_equal"] = torch.equal(part, full[pick])
         res["unet_exchanges"] = dict(vs.exchanges)
 
         dec, _ = _build_decoder()
-        Pd = dec._pack(torch.device("cpu"))
         z = torch.randn(T, 4, 8, 8, generator=torch.Generator().manual_seed(3))
-        full_d = dec._run(Pd, z, T, T, 1, 8, 8)
+        full_d = dec(z, timesteps=T)
         dec.view_shard = vs
         try:
-            part_d = dec._run(Pd, z[vs.frames].contiguous(), vs.tl, vs.tl, 1, 8, 8)
+            part_d = dec(z[vs.frames].contiguous(), timesteps=vs.tl)
         finally:
             dec.view_shard = None
         res["dec_equal"] = torch.equal(vs.gather_frames(part_d), full_d)

@@ -35,14 +35,16 @@ def _params(m):
     return {k: m[k] for k in ("eta", "s_noise", "order") if m.get(k) is not None}
 
 
-def _dropin(shim_cls, m, T, **over):
+def _dropin(name, m, T, **over):
+    from v3d_b200 import sampling
+
     kw = dict(num_steps=m["num_steps"],
               discretization_config={"target": BASE + "discretizer.EDMDiscretization",
                                      "params": {"sigma_max": m["sigma_max"]}},
               guider_config={"target": BASE + "guiders.LinearPredictionGuider",
                              "params": {"max_scale": m["max_scale"], "min_scale": m["min_scale"], "num_frames": T}})
     kw.update(_params(m), **over)
-    return shim_cls(**kw)
+    return getattr(sampling, name)(**kw)
 
 
 def _counting(fn, box):
@@ -89,7 +91,6 @@ def test_dropin_logic_exact_with_fp32_network(tag):
     """The drop-in samplers (step kernels as stand-ins) around the ORACLE's fp32 UNet reproduce the real reference's
     outputs to fp32 rounding: schedule, multipliers, skipped evaluations, history and the injected noise, in order.
     They also evaluate the network exactly as often as the reference did."""
-    import cpu_shims
     import emu_ops
     from oracle import make_golden_samplers as mgs
     from oracle import ref_unet, synth
@@ -101,7 +102,7 @@ def test_dropin_logic_exact_with_fp32_network(tag):
     sd = synth.synth_state_dict(ref_unet.unet_param_shapes(spec), seed=mu["weight_seed"])
     T, hw = m["T"], m["latent_hw"]
     x, c, uc = synth.synth_inputs(T, hw)
-    sampler = _dropin(cpu_shims.CPU_SHIMS[m["sampler"]], m, T)
+    sampler = _dropin(m["sampler"], m, T)
     if m.get("noise_seed") is not None:
         sampler.noise_sampler = mgs.seeded_noise(m["noise_seed"])
     den = sampling.Denoiser({"target": BASE + "denoiser_scaling.VScalingWithEDMcNoise"})
@@ -125,7 +126,6 @@ def test_dropin_logic_exact_with_fp32_network(tag):
 def test_dropin_host_path_with_bf16_unet_matches_reference_golden(tag):
     """The drop-in samplers through the drop-in Denoiser / OpenAIWrapper / VideoUNet host schedule with every kernel
     as its CPU stand-in (bf16 network), against the real reference's fp32 outputs: the GPU parity bound, rel-L2 3e-2."""
-    import cpu_shims
     import emu_ops
     from oracle import make_golden_samplers as mgs
     from oracle import synth
@@ -136,10 +136,9 @@ def test_dropin_host_path_with_bf16_unet_matches_reference_golden(tag):
     gold = torch.load(GOLD / f"{tag}.pt")
     net = VideoUNet(**dict(UNET_KW, model_channels=mu["model_channels"]))
     net.load_state_dict(synth.synth_state_dict(net.param_shapes(), seed=mu["weight_seed"]), strict=True)
-    net.__class__ = cpu_shims.CpuUNet
     T, hw = m["T"], m["latent_hw"]
     x, c, uc = synth.synth_inputs(T, hw)
-    sampler = _dropin(cpu_shims.CPU_SHIMS[m["sampler"]], m, T)
+    sampler = _dropin(m["sampler"], m, T)
     if m.get("noise_seed") is not None:
         sampler.noise_sampler = mgs.seeded_noise(m["noise_seed"])
     den = sampling.Denoiser({"target": BASE + "denoiser_scaling.VScalingWithEDMcNoise"})
@@ -174,14 +173,14 @@ def test_noise_calls_and_network_evaluations(name):
     network runs N times for N steps (DPM++ 2S: 2N - 1, the last step has no midpoint).  sigma_max 80 keeps every
     sigma_down of this schedule nonzero in fp32 (a step from 700 straight down to 0.002 rounds it to exactly 0, and the
     reference then skips that midpoint too)."""
-    import cpu_shims
     import emu_ops
+    from v3d_b200 import sampling
 
     T, hw, steps = 3, 4, 4
-    sampler = cpu_shims.CPU_SHIMS[name](num_steps=steps,
-                                        discretization_config={"target": BASE + "discretizer.EDMDiscretization"},
-                                        guider_config={"target": BASE + "guiders.LinearPredictionGuider",
-                                                       "params": {"max_scale": 2.5, "num_frames": T}})
+    sampler = getattr(sampling, name)(num_steps=steps,
+                                      discretization_config={"target": BASE + "discretizer.EDMDiscretization"},
+                                      guider_config={"target": BASE + "guiders.LinearPredictionGuider",
+                                                     "params": {"max_scale": 2.5, "num_frames": T}})
     calls = []
     if hasattr(sampler, "noise_sampler"):
         default = sampler.noise_sampler
@@ -239,6 +238,7 @@ def test_ancestral_step_helpers_match_reference_formulas():
 @pytest.mark.parametrize("name", ["EulerAncestralSampler", "DPMPP2SAncestralSampler"])
 def test_eta_zero_is_refused(name):
     """The reference fails at the first ancestral step with eta = 0; the drop-ins refuse it with a clear error."""
+    import emu_ops
     from v3d_b200 import sampling
 
     disc = {"target": BASE + "discretizer.EDMDiscretization"}
@@ -246,8 +246,10 @@ def test_eta_zero_is_refused(name):
         getattr(sampling, name)(eta=0.0, num_steps=2, discretization_config=disc)
     smp = getattr(sampling, name)(num_steps=2, discretization_config=disc)
     smp.eta = 0
-    with pytest.raises(ValueError, match="eta = 0"):
-        smp._loop(lambda i, s, c: i, torch.zeros(1, 4, 2, 2), {})
+    with pytest.raises(ValueError, match="eta = 0"), emu_ops.patched() as launches:
+        n0 = sum(launches.values())
+        smp(lambda i, s, c: i, torch.zeros(1, 4, 2, 2), {})
+    assert sum(launches.values()) == n0
 
 
 def test_lms_order_above_eight_is_refused():
@@ -259,14 +261,67 @@ def test_lms_order_above_eight_is_refused():
         sampling.LinearMultistepSampler(order=9, num_steps=2, discretization_config=disc)
 
 
+SAMPLER_NAMES = ["EulerEDMSampler", "HeunEDMSampler", "EulerAncestralSampler", "DPMPP2SAncestralSampler",
+                 "DPMPP2MSampler", "LinearMultistepSampler"]
+
+
 def test_cuda_only():
+    """Without the stand-ins every sampler and module refuses CPU tensors at its one gate, before any work."""
+    from test_host_schedule_cpu import DEC_KW, _build_unet, _unet, _unet_inputs
     from v3d_b200 import sampling
+    from v3d_b200.decoder import VideoDecoder
+    from v3d_b200.encoder import Encoder
 
     disc = {"target": BASE + "discretizer.EDMDiscretization"}
-    for name in ("EulerAncestralSampler", "DPMPP2SAncestralSampler", "DPMPP2MSampler", "LinearMultistepSampler"):
-        with pytest.raises(RuntimeError, match="needs CUDA tensors"):
-            getattr(sampling, name)(num_steps=2, discretization_config=disc)(lambda i, s, c: i, torch.zeros(1, 4, 2, 2),
-                                                                              {})
+    for name in SAMPLER_NAMES:
+        x = torch.ones(1, 4, 2, 2)
+        with pytest.raises(RuntimeError, match="needs CUDA tensors.*no CPU fallback"):
+            getattr(sampling, name)(num_steps=2, discretization_config=disc)(lambda i, s, c: i, x, {})
+        assert (x == 1).all()                                   # refused before the noise is scaled in place
+    net, _ = _build_unet()
+    with pytest.raises(RuntimeError, match="VideoUNet.forward needs CUDA tensors.*no CPU fallback"):
+        _unet(net, *_unet_inputs(2, 8), 2)
+    dec = VideoDecoder(**DEC_KW)
+    with pytest.raises(RuntimeError, match="VideoDecoder.forward needs CUDA tensors.*no CPU fallback"):
+        dec(torch.zeros(2, 4, 8, 8), timesteps=2)
+    enc = Encoder(double_z=True, z_channels=4, resolution=256, in_channels=3, out_ch=3, ch=64, ch_mult=[1, 2, 4, 4],
+                  num_res_blocks=2, attn_resolutions=[], dropout=0.0, attn_type="vanilla")
+    with pytest.raises(RuntimeError, match="Encoder.forward needs CUDA tensors.*no CPU fallback"):
+        enc(torch.zeros(1, 3, 64, 64))
+    for mod in (net, dec, enc):
+        assert mod._packed is None
+        with pytest.raises(RuntimeError, match="packed needs CUDA tensors.*no CPU fallback"):
+            mod.packed()
+
+
+# (ops calls, sha256 of the launch record) of 3 steps of each sampler around an identity denoiser, LinearPrediction
+# guider over 3 frames, recorded when the CPU suite still ran the samplers through test-only subclasses
+SAMPLER_LAUNCHES = {
+    "EulerEDMSampler": (6, "b2f0e77d11f85792a37839abb22ce1fc9b589a3c09ceadd0035d7774435a6528"),
+    "HeunEDMSampler": (10, "e6c2de924c11fa9a0c8127314d4ca8236622303ea1eefd9305f68e3dfad70090"),
+    "EulerAncestralSampler": (6, "08a310b2bbd5ff111f78d288b6697ebb6e125c2f9435e75806951723bbd20ef6"),
+    "DPMPP2SAncestralSampler": (10, "b3dae46b9cdc99035924013c23a209c1768c5c585893c6b42b8f73013f8118ac"),
+    "DPMPP2MSampler": (6, "b1fe1a0d4114a903cf8c7365bde0f10e8e9ea0b9f9de12a0bfd7fd27819244ab"),
+    "LinearMultistepSampler": (6, "ff373080758c1247238fa6b120a3a67f32d7f5bd841ed4e16bb90ceaf9e98583"),
+}
+
+
+@pytest.mark.parametrize("name", SAMPLER_NAMES)
+def test_sampler_launch_sequence_is_unchanged(name):
+    import emu_ops
+    from v3d_b200 import sampling
+
+    T = 3
+    smp = getattr(sampling, name)(num_steps=3, discretization_config={"target": BASE + "discretizer.EDMDiscretization"},
+                                  guider_config={"target": BASE + "guiders.LinearPredictionGuider",
+                                                 "params": {"max_scale": 2.5, "num_frames": T}})
+    g = torch.Generator().manual_seed(0)
+    x = torch.randn(T, 4, 4, 4, generator=g)
+    c = {"crossattn": torch.randn(T, 1, 8, generator=g), "vector": torch.randn(T, 8, generator=g)}
+    calls = []
+    with emu_ops.patched(calls):
+        smp(lambda i, s, cc: i, x, cond=c, uc={k: 0 * v for k, v in c.items()})
+    assert emu_ops.digest(calls) == SAMPLER_LAUNCHES[name], emu_ops.digest(calls)
 
 
 def test_targets_resolve():

@@ -32,6 +32,7 @@ import torch.nn.functional as F
 
 from . import ops
 from .sampling import instantiate_from_config
+from .unet import KernelModule
 
 CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)
 CLIP_STD = (0.26862954, 0.26130258, 0.27577711)
@@ -82,7 +83,7 @@ class _OpenClipShell(nn.Module):
             p.requires_grad_(False)
 
 
-class FrozenOpenCLIPImageEmbedder(nn.Module):
+class FrozenOpenCLIPImageEmbedder(KernelModule):
     """encoders/modules.py:594-752 for the configuration V3D uses (configs/embedder/clip_image.yaml: freeze, every
     other option at its default).  Options that change the output structure raise at construction."""
 
@@ -98,16 +99,10 @@ class FrozenOpenCLIPImageEmbedder(nn.Module):
         self.antialias, self.ucg_rate, self.unsqueeze_dim, self.max_length = antialias, ucg_rate, unsqueeze_dim, max_length
         self.register_buffer("mean", torch.tensor(CLIP_MEAN), persistent=False)
         self.register_buffer("std", torch.tensor(CLIP_STD), persistent=False)
-        self._packed = None
-        self.register_load_state_dict_post_hook(_drop_pack)
 
     def freeze(self):
         self.eval()
         return self
-
-    def _apply(self, fn, *a, **kw):
-        self._packed = None
-        return super()._apply(fn, *a, **kw)
 
     # ---- preprocessing (encoders/modules.py:645-657; kornia.geometry.resize restated, see oracle/ref_clip.py) -------
     def preprocess(self, x: torch.Tensor) -> torch.Tensor:
@@ -130,39 +125,33 @@ class FrozenOpenCLIPImageEmbedder(nn.Module):
         x = (x + 1.0) / 2.0
         return (x - self.mean.view(1, 3, 1, 1)) / self.std.view(1, 3, 1, 1)
 
-    # ---- weights: bf16 operands packed once ------------------------------------------------------------------------
-    def packed(self) -> dict:
-        if self._packed is None:
-            v = self.model.visual
-            dev = v.proj.device
-            bf = lambda t: t.detach().to(torch.bfloat16).contiguous()       # noqa: E731
-            f32 = lambda t: t.detach().float().contiguous()                 # noqa: E731
-            kp = v.patch * v.patch * 3
-            kpad = (kp + 63) // 64 * 64
-            w1 = torch.zeros(v.width, kpad, device=dev)
-            w1[:, :kp] = v.conv1.weight.detach().reshape(v.width, kp)       # (c, ky, kx) order = F.unfold's
-            P = {"conv1": bf(w1), "kpad": kpad, "kp": kp, "cls": f32(v.class_embedding), "pos": f32(v.positional_embedding),
-                 "ln_pre": (f32(v.ln_pre.weight), f32(v.ln_pre.bias)), "ln_post": (f32(v.ln_post.weight), f32(v.ln_post.bias)),
-                 "proj_t": bf(v.proj.detach().t()), "blocks": []}
-            bn = ops.pick_block_n(2 * v.mlp, ops.ACT_GEGLU)
-            perm = ops.geglu_perm(v.mlp, bn).to(dev)
-            for blk in v.transformer.resblocks:
-                fc_w = torch.cat([torch.zeros_like(blk.mlp.c_fc.weight), blk.mlp.c_fc.weight.detach()], 0)[perm]
-                fc_b = torch.cat([torch.ones_like(blk.mlp.c_fc.bias), blk.mlp.c_fc.bias.detach()], 0)[perm]
-                P["blocks"].append({
-                    "ln1": (f32(blk.ln_1.weight), f32(blk.ln_1.bias)), "ln2": (f32(blk.ln_2.weight), f32(blk.ln_2.bias)),
-                    "qkv_w": bf(blk.attn.in_proj_weight), "qkv_b": f32(blk.attn.in_proj_bias),
-                    "out_w": bf(blk.attn.out_proj.weight), "out_b": f32(blk.attn.out_proj.bias),
-                    "fc_w": bf(fc_w), "fc_b": f32(fc_b),
-                    "proj_w": bf(blk.mlp.c_proj.weight), "proj_b": f32(blk.mlp.c_proj.bias)})
-            self._packed = P
-        return self._packed
+    # ---- weights: bf16 operands packed once (KernelModule.packed) -------------------------------------------------
+    def _pack(self, dev: torch.device) -> dict:
+        v, bf, f32 = self.model.visual, self._bf, self._f32
+        kp = v.patch * v.patch * 3
+        kpad = (kp + 63) // 64 * 64
+        w1 = torch.zeros(v.width, kpad, device=dev)
+        w1[:, :kp] = v.conv1.weight.detach().reshape(v.width, kp)       # (c, ky, kx) order = F.unfold's
+        P = {"conv1": bf(w1), "kpad": kpad, "kp": kp, "cls": f32(v.class_embedding), "pos": f32(v.positional_embedding),
+             "ln_pre": (f32(v.ln_pre.weight), f32(v.ln_pre.bias)), "ln_post": (f32(v.ln_post.weight), f32(v.ln_post.bias)),
+             "proj_t": bf(v.proj.detach().t()), "blocks": []}
+        bn = ops.pick_block_n(2 * v.mlp, ops.ACT_GEGLU)
+        perm = ops.geglu_perm(v.mlp, bn).to(dev)
+        for blk in v.transformer.resblocks:
+            fc_w = torch.cat([torch.zeros_like(blk.mlp.c_fc.weight), blk.mlp.c_fc.weight.detach()], 0)[perm]
+            fc_b = torch.cat([torch.ones_like(blk.mlp.c_fc.bias), blk.mlp.c_fc.bias.detach()], 0)[perm]
+            P["blocks"].append({
+                "ln1": (f32(blk.ln_1.weight), f32(blk.ln_1.bias)), "ln2": (f32(blk.ln_2.weight), f32(blk.ln_2.bias)),
+                "qkv_w": bf(blk.attn.in_proj_weight), "qkv_b": f32(blk.attn.in_proj_bias),
+                "out_w": bf(blk.attn.out_proj.weight), "out_b": f32(blk.attn.out_proj.bias),
+                "fc_w": bf(fc_w), "fc_b": f32(fc_b),
+                "proj_w": bf(blk.mlp.c_proj.weight), "proj_b": f32(blk.mlp.c_proj.bias)})
+        return P
 
     # ---- the tower ---------------------------------------------------------------------------------------------------
     @torch.no_grad()
     def encode_with_vision_transformer(self, img: torch.Tensor) -> torch.Tensor:
-        if not img.is_cuda:
-            raise RuntimeError("v3d_b200 FrozenOpenCLIPImageEmbedder needs CUDA tensors; there is no CPU fallback")
+        ops.require_current_device(img, "v3d_b200.FrozenOpenCLIPImageEmbedder")
         v, P = self.model.visual, self.packed()
         dev = img.device
         x = self.preprocess(img)
@@ -229,10 +218,6 @@ class FrozenOpenCLIPImageEmbedder(nn.Module):
 
     def encode(self, image):
         return self(image)
-
-
-def _drop_pack(module, incompatible_keys):
-    module._packed = None
 
 
 class FrozenOpenCLIPImagePredictionEmbedder(nn.Module):

@@ -267,8 +267,6 @@ class VideoDecoder(KernelModule):
     def forward(self, z: torch.Tensor, timesteps: Optional[int] = None, skip_video: bool = False, **kwargs):
         if skip_video:
             raise NotImplementedError("skip_video decode is not implemented")
-        if not z.is_cuda:
-            raise RuntimeError("v3d_b200.VideoDecoder.forward needs CUDA tensors; there is no CPU fallback")
         ops.require_current_device(z, "v3d_b200.VideoDecoder.forward")
         B, zc, H, W = z.shape
         T = int(timesteps) if timesteps else B

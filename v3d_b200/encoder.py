@@ -193,8 +193,6 @@ class Encoder(KernelModule):
         return out, ho, wo
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if not x.is_cuda:
-            raise RuntimeError("v3d_b200.Encoder.forward needs CUDA tensors; there is no CPU fallback")
         ops.require_current_device(x, "v3d_b200.Encoder.forward")
         assert x.shape[1] == self.in_channels
         with torch.no_grad():

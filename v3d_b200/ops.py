@@ -34,10 +34,13 @@ def _need(t: torch.Tensor, dtype, name: str) -> None:
 
 
 def require_current_device(t: torch.Tensor, who: str) -> None:
-    """The library launches on the CURRENT device's current stream and caches per-device kernel attributes per process
-    (one process per GPU is the deployment model): a tensor on another device would be launched on the wrong stream.
-    Called once per forward by the modules."""
-    if t.is_cuda and t.device.index != torch.cuda.current_device():
+    """The one refusal of the package's entry points: every module forward, sampler call and weight packing calls it
+    once.  There is no CPU path, so a tensor that is not on CUDA is refused.  The library launches on the CURRENT
+    device's current stream and caches per-device kernel attributes per process (one process per GPU is the deployment
+    model): a tensor on another device would be launched on the wrong stream, so it is refused too."""
+    if not t.is_cuda:
+        raise RuntimeError(f"{who} needs CUDA tensors (got {t.device}); there is no CPU fallback")
+    if t.device.index != torch.cuda.current_device():
         raise RuntimeError(f"{who}: tensor on cuda:{t.device.index} but the current device is cuda:"
                            f"{torch.cuda.current_device()}; call torch.cuda.set_device(...) first (one process per GPU)")
 

@@ -232,116 +232,6 @@ class IdentityGuider:
         return x, s, {k: c[k] for k in c}
 
 
-class EulerEDMSampler:
-    """EDM Euler sampler (sampling.py:24-133,214-218). s_churn > 0 (noise injection) keeps the reference
-    semantics via torch.randn_like; V3D_512 runs with s_churn = 0."""
-
-    def __init__(self, discretization_config, num_steps: Optional[int] = None, guider_config=None,
-                 verbose: bool = False, device: str = "cuda", s_churn: float = 0.0, s_tmin: float = 0.0,
-                 s_tmax: float = float("inf"), s_noise: float = 1.0):
-        self.num_steps = num_steps
-        self.discretization = instantiate_from_config(discretization_config)
-        self.guider = instantiate_from_config(guider_config if guider_config is not None else DEFAULT_GUIDER)
-        self.verbose = verbose
-        self.device = device
-        self.s_churn, self.s_tmin, self.s_tmax, self.s_noise = s_churn, s_tmin, s_tmax, s_noise
-
-    def prepare_sampling_loop(self, x, cond, uc=None, num_steps=None):
-        sigmas = self.discretization(self.num_steps if num_steps is None else num_steps, device="cpu")
-        uc = cond if uc is None else uc
-        x *= float(torch.sqrt(1.0 + sigmas[0] ** 2.0))  # in place on the caller's noise, like sampling.py:50
-        return x, sigmas, len(sigmas), cond, uc
-
-    def denoise(self, x, denoiser, sigma, cond, uc):
-        denoised = denoiser(*self.guider.prepare_inputs(x, sigma, cond, uc))
-        return self.guider(denoised, sigma)
-
-    def possible_correction_step(self, euler_step, x, d, dt, next_sigma, denoiser, cond, uc):
-        return euler_step
-
-    def sampler_step(self, sigma, next_sigma, denoiser, x, cond, uc=None, gamma: float = 0.0):
-        sigma_hat = sigma if gamma == 0 else sigma * (gamma + 1.0)
-        if gamma > 0:
-            eps = torch.randn_like(x) * self.s_noise
-            x = x + eps * (sigma_hat ** 2 - sigma ** 2).reshape(-1, *([1] * (x.ndim - 1))) ** 0.5
-        denoised = self.denoise(x, denoiser, sigma_hat, cond, uc).float().contiguous()
-        out = torch.empty_like(x)
-        ops.euler_step(x, denoised, sigma_hat, next_sigma, out, x.shape[0], x[0].numel())
-        return out
-
-    def __call__(self, denoiser, x, cond, uc=None, num_steps=None):
-        if not x.is_cuda:
-            raise RuntimeError("v3d_b200.EulerEDMSampler needs CUDA tensors; there is no CPU fallback")
-        return self._loop(denoiser, x, cond, uc, num_steps)
-
-    def _loop(self, denoiser, x, cond, uc=None, num_steps=None):
-        """EDMSampler.__call__ (sampling.py:112-133) below the CUDA check."""
-        assert x.dtype == torch.float32, "sampler state is fp32 (denoiser.py:36-39)"
-        x, sigmas, num_sigmas, cond, uc = self.prepare_sampling_loop(x, cond, uc, num_steps)
-        n = x.shape[0]
-        # per-step sigma vectors built once (one small H2D copy), indexed on the host
-        sig_rows = sigmas.float().reshape(-1, 1).expand(num_sigmas, n).contiguous().to(x.device)
-        host = [float(s) for s in sigmas]
-        steps = range(num_sigmas - 1)
-        if self.verbose:
-            from tqdm import tqdm
-
-            steps = tqdm(steps, total=num_sigmas - 1, desc=f"Sampling with {type(self).__name__}")
-        x = x.contiguous()
-        for i in steps:
-            gamma = min(self.s_churn / (num_sigmas - 1), 2 ** 0.5 - 1) if self.s_tmin <= host[i] <= self.s_tmax else 0.0
-            x = self.sampler_step(sig_rows[i], sig_rows[i + 1], denoiser, x, cond, uc, gamma)
-        return x
-
-
-class HeunEDMSampler(EulerEDMSampler):
-    """Second-order EDM sampler (sampling.py:221-237): after the Euler proposal the denoiser is evaluated once more at
-    sigma_next and the step is redone with the averaged slope; the last step (sigma_next = 0) stays first order, which
-    also saves the network evaluation exactly as the reference does (`torch.sum(next_sigma) < 1e-14`)."""
-
-    _next_sigma_host: Optional[float] = None  # set by __call__: lets the step skip the device->host sync
-
-    def sampler_step(self, sigma, next_sigma, denoiser, x, cond, uc=None, gamma: float = 0.0):
-        sigma_hat = sigma if gamma == 0 else sigma * (gamma + 1.0)
-        if gamma > 0:
-            eps = torch.randn_like(x) * self.s_noise
-            x = x + eps * (sigma_hat ** 2 - sigma ** 2).reshape(-1, *([1] * (x.ndim - 1))) ** 0.5
-        n, per = x.shape[0], x[0].numel()
-        denoised = self.denoise(x, denoiser, sigma_hat, cond, uc).float().contiguous()
-        x_euler = torch.empty_like(x)
-        ops.euler_step(x, denoised, sigma_hat, next_sigma, x_euler, n, per)
-        nsum = self._next_sigma_host if self._next_sigma_host is not None else float(next_sigma.sum())
-        if nsum < 1e-14:
-            return x_euler
-        denoised2 = self.denoise(x_euler, denoiser, next_sigma, cond, uc).float().contiguous()
-        out = torch.empty_like(x)
-        ops.heun_step(x, denoised, x_euler, denoised2, sigma_hat.float().contiguous(),
-                      next_sigma.float().contiguous(), out, n, per)
-        return out
-
-    def __call__(self, denoiser, x, cond, uc=None, num_steps=None):
-        if not x.is_cuda:
-            raise RuntimeError("v3d_b200.HeunEDMSampler needs CUDA tensors; there is no CPU fallback")
-        return self._loop(denoiser, x, cond, uc, num_steps)
-
-    def _loop(self, denoiser, x, cond, uc=None, num_steps=None):
-        assert x.dtype == torch.float32, "sampler state is fp32 (denoiser.py:36-39)"
-        x, sigmas, num_sigmas, cond, uc = self.prepare_sampling_loop(x, cond, uc, num_steps)
-        n = x.shape[0]
-        sig_rows = sigmas.float().reshape(-1, 1).expand(num_sigmas, n).contiguous().to(x.device)
-        host = [float(s) for s in sigmas]
-        x = x.contiguous()
-        try:
-            for i in range(num_sigmas - 1):
-                gamma = (min(self.s_churn / (num_sigmas - 1), 2 ** 0.5 - 1)
-                         if self.s_tmin <= host[i] <= self.s_tmax else 0.0)
-                self._next_sigma_host = host[i + 1] * n
-                x = self.sampler_step(sig_rows[i], sig_rows[i + 1], denoiser, x, cond, uc, gamma)
-        finally:
-            self._next_sigma_host = None
-        return x
-
-
 # ---------------------------------------------------------------------------------------------------------------------
 # sampling_utils.py:7-43 (also exported at v3d_b200.sgm.modules.diffusionmodules.sampling_utils)
 # ---------------------------------------------------------------------------------------------------------------------
@@ -425,7 +315,11 @@ class _ScheduleSampler:
         self.verbose = verbose
         self.device = device
 
-    prepare_sampling_loop = EulerEDMSampler.prepare_sampling_loop
+    def prepare_sampling_loop(self, x, cond, uc=None, num_steps=None):
+        sigmas = self.discretization(self.num_steps if num_steps is None else num_steps, device="cpu")
+        uc = cond if uc is None else uc
+        x *= float(torch.sqrt(1.0 + sigmas[0] ** 2.0))  # in place on the caller's noise, like sampling.py:50
+        return x, sigmas, len(sigmas), cond, uc
 
     def denoise(self, x, denoiser, sigma, cond, uc, **kwargs):
         denoised = denoiser(*self.guider.prepare_inputs(x, sigma, cond, uc), **kwargs)
@@ -440,14 +334,86 @@ class _ScheduleSampler:
         return steps
 
     def __call__(self, denoiser, x, cond, uc=None, num_steps=None, **kwargs):
-        if not x.is_cuda:
-            raise RuntimeError(f"v3d_b200.{type(self).__name__} needs CUDA tensors; there is no CPU fallback")
+        ops.require_current_device(x, f"v3d_b200.{type(self).__name__}")
         return self._loop(denoiser, x, cond, uc, num_steps, **kwargs)
 
     def _start(self, x, cond, uc, num_steps):
         assert x.dtype == torch.float32, "sampler state is fp32 (denoiser.py:36-39)"
         x, sigmas, num_sigmas, cond, uc = self.prepare_sampling_loop(x, cond, uc, num_steps)
         return x.contiguous(), sigmas.float(), num_sigmas, cond, uc
+
+
+class EulerEDMSampler(_ScheduleSampler):
+    """EDM Euler sampler (sampling.py:24-133,214-218). s_churn > 0 (noise injection) keeps the reference
+    semantics via torch.randn_like; V3D_512 runs with s_churn = 0."""
+
+    def __init__(self, discretization_config, num_steps: Optional[int] = None, guider_config=None,
+                 verbose: bool = False, device: str = "cuda", s_churn: float = 0.0, s_tmin: float = 0.0,
+                 s_tmax: float = float("inf"), s_noise: float = 1.0):
+        super().__init__(discretization_config, num_steps, guider_config, verbose, device)
+        self.s_churn, self.s_tmin, self.s_tmax, self.s_noise = s_churn, s_tmin, s_tmax, s_noise
+
+    def possible_correction_step(self, euler_step, x, d, dt, next_sigma, denoiser, cond, uc):
+        return euler_step
+
+    def _churn(self, x, sigma, gamma: float):
+        """-> (x, sigma_hat): the state with the churn noise added and the raised sigma (sampling.py:97-101)."""
+        sigma_hat = sigma if gamma == 0 else sigma * (gamma + 1.0)
+        if gamma > 0:
+            eps = torch.randn_like(x) * self.s_noise
+            x = x + eps * (sigma_hat ** 2 - sigma ** 2).reshape(-1, *([1] * (x.ndim - 1))) ** 0.5
+        return x, sigma_hat
+
+    def sampler_step(self, sigma, next_sigma, denoiser, x, cond, uc=None, gamma: float = 0.0):
+        x, sigma_hat = self._churn(x, sigma, gamma)
+        denoised = self.denoise(x, denoiser, sigma_hat, cond, uc)
+        out = torch.empty_like(x)
+        ops.euler_step(x, denoised, sigma_hat, next_sigma, out, x.shape[0], x[0].numel())
+        return out
+
+    def _loop(self, denoiser, x, cond, uc=None, num_steps=None):
+        """EDMSampler.__call__ (sampling.py:112-133)."""
+        x, sigmas, num_sigmas, cond, uc = self._start(x, cond, uc, num_steps)
+        n = x.shape[0]
+        host = [float(s) for s in sigmas]
+        rows = _sigma_rows(host, n, x.device)
+        for i in self._steps(num_sigmas):
+            gamma = min(self.s_churn / (num_sigmas - 1), 2 ** 0.5 - 1) if self.s_tmin <= host[i] <= self.s_tmax else 0.0
+            x = self._step(host[i + 1] * n, rows[i], rows[i + 1], denoiser, x, cond, uc, gamma)
+        return x
+
+    def _step(self, next_sigma_sum: float, *step_args):
+        return self.sampler_step(*step_args)
+
+
+class HeunEDMSampler(EulerEDMSampler):
+    """Second-order EDM sampler (sampling.py:221-237): after the Euler proposal the denoiser is evaluated once more at
+    sigma_next and the step is redone with the averaged slope; the last step (sigma_next = 0) stays first order, which
+    also saves the network evaluation exactly as the reference does (`torch.sum(next_sigma) < 1e-14`)."""
+
+    _next_sigma_host: Optional[float] = None  # set by _step: lets the step skip the device->host sync
+
+    def sampler_step(self, sigma, next_sigma, denoiser, x, cond, uc=None, gamma: float = 0.0):
+        x, sigma_hat = self._churn(x, sigma, gamma)
+        n, per = x.shape[0], x[0].numel()
+        denoised = self.denoise(x, denoiser, sigma_hat, cond, uc)
+        x_euler = torch.empty_like(x)
+        ops.euler_step(x, denoised, sigma_hat, next_sigma, x_euler, n, per)
+        nsum = self._next_sigma_host if self._next_sigma_host is not None else float(next_sigma.sum())
+        if nsum < 1e-14:
+            return x_euler
+        denoised2 = self.denoise(x_euler, denoiser, next_sigma, cond, uc)
+        out = torch.empty_like(x)
+        ops.heun_step(x, denoised, x_euler, denoised2, sigma_hat.float().contiguous(),
+                      next_sigma.float().contiguous(), out, n, per)
+        return out
+
+    def _step(self, next_sigma_sum: float, *step_args):
+        self._next_sigma_host = next_sigma_sum
+        try:
+            return self.sampler_step(*step_args)
+        finally:
+            self._next_sigma_host = None
 
 
 class _AncestralSampler(_ScheduleSampler):

@@ -81,17 +81,12 @@ class KernelModule(nn.Module):
         self._invalidate()
         return super()._apply(fn, recurse)
 
-    def _device(self) -> torch.device:
-        return next(self.parameters()).device
-
     def packed(self) -> dict:
         if self._packed is None:
-            dev = self._device()
-            if dev.type != "cuda":
-                raise RuntimeError(f"{type(self).__name__} runs on CUDA only (parameters are on {dev}); "
-                                   "there is no CPU fallback")
+            p = next(self.parameters())
+            ops.require_current_device(p, f"v3d_b200.{type(self).__name__}.packed")
             with torch.no_grad():
-                self._packed = self._pack(dev)
+                self._packed = self._pack(p.device)
         return self._packed
 
     def _pack(self, dev: torch.device) -> dict:  # pragma: no cover - abstract
@@ -723,8 +718,6 @@ class VideoUNet(KernelModule):
         num_video_frames: Optional[int] = None,
         image_only_indicator: Optional[torch.Tensor] = None,
     ) -> torch.Tensor:
-        if not x.is_cuda:
-            raise RuntimeError("v3d_b200.VideoUNet.forward needs CUDA tensors; there is no CPU fallback")
         ops.require_current_device(x, "v3d_b200.VideoUNet.forward")
         args, dims, graphs = self._prepare(x, timesteps, context, y, time_context, num_video_frames,
                                            image_only_indicator)
@@ -761,7 +754,7 @@ class VideoUNet(KernelModule):
         self._check_indicator(image_only_indicator, nb, T)
         dev = x.device
         ctx2d = context.float().reshape(B, -1)
-        graphs = self.cuda_graphs
+        graphs = self.cuda_graphs and x.is_cuda          # capture needs CUDA inputs (tests run forward on CPU)
         if vs is not None:
             # frame-sharded call: x / context / y hold this rank's T = vs.tl frames of each video; the temporal
             # cross-attention context (frame 0 of each video, video_attention.py:250) may live on another rank and

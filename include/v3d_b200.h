@@ -56,7 +56,10 @@ int64_t v3d_launch_count(void);
  *            replaces nn.Conv2d 3x3 s1 p1: openaimodel.py:145-147,267-315; video_model.py:189,439;
  *            model.py:65-66,111-120,651-653.
  * B is always [N][ntaps*K] (K-major, tap-major then channel), optionally batched.
- * All of K, lda, ldb, ldd, ldr* are in elements; K % 64 == 0; N % 16 == 0.
+ * All of K, lda, ldb, ldd, ldr* are in elements; K % 64 == 0; N % 16 == 0; lda, ldb, ldd % 8 == 0.
+ * A residual needs an even ldr* and a 4-byte aligned base.  With a 16-byte aligned base and ldr* % 8 == 0 (the
+ * usual case) the bf16-output epilogues load it into shared memory by TMA during the main loop; otherwise the
+ * epilogue reads it from global memory.  Both give the same bits.
  * ------------------------------------------------------------------------------------------ */
 typedef struct v3d_gemm_args {
   const void* A;      /* bf16 */

@@ -2,6 +2,9 @@
 //
 // One persistent, warp-specialised kernel, 128 x BN output tiles:
 //   warpgroup 0    : TMA producer (one thread; A tile 128x64 bf16 + B tile BNx64 bf16 per pipeline stage, 128B swizzle)
+//                    and, for the bf16 epilogues, one epilogue I/O thread (warp 1): it loads each tile's residual
+//                    sub-tiles into the staging buffer by TMA while the consumers still run the tile's main loop, and
+//                    writes the finished tile out of the same buffer by TMA.
 //   warpgroups 1-2 : consumers.  Each owns 64 rows of the tile: wgmma.mma_async m64nBNk16 from shared memory into
 //                    fp32 register accumulators, then the epilogue straight from those registers (bias / per-frame
 //                    bias / SiLU / GEGLU / residual blend -> bf16 sub-tiles staged in shared memory and written by TMA,
@@ -11,6 +14,7 @@
 // The im2row never exists in memory: each (tap, 64-channel) K-block is one TMA box whose out-of-bounds
 // part is zero-filled by the hardware, which is exactly the conv zero padding.
 #include <cstdlib>
+#include <type_traits>
 
 #include "common.cuh"
 #include "host_util.cuh"
@@ -42,11 +46,14 @@ struct GemmEpi {
   int num_m_tiles, num_n_tiles;
   float s0, s1, s2;
   int tap0;  // A row coordinate of tap 0 relative to the output row: a_row0 - (ntaps / 2) * tap_shift
+  // residuals fetched into shared memory by TMA (mapR1 / mapR2) instead of __ldg from the epilogue: every residual's
+  // base and row pitch are 16-byte aligned.  R2 is staged only by the variants that have room for it (Cfg::R2_STAGED).
+  int res_tma;
 };
 
 // Fused GEMM -> all-gather over peer memory: output sub-tiles whose first column is >= col0 are stored a second time
 // through each of these tensor maps (destination matrices that may live on other GPUs: IPC-mapped arenas), by the same
-// store leader with the same cp.async.bulk.tensor instruction.  n = 0: off (every launch but the frame-sharded K|V
+// epilogue I/O thread with the same cp.async.bulk.tensor instruction.  n = 0: off (every launch but the frame-sharded K|V
 // projection).
 struct alignas(64) KvMaps {
   CUtensorMap m[8];
@@ -72,7 +79,12 @@ struct Cfg {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGING_BYTES = STAGED ? NSUB * SUB_BYTES : 0;
+  static constexpr int TILE_OUT_BYTES = NSUB * SUB_BYTES;
+  // R2 takes a second staging buffer, but only where the operand ring keeps at least 4 stages with it (BN <= 160);
+  // BN = 256 would drop to 2 stages, so there R2 stays an __ldg from the epilogue.
+  static constexpr bool R2_STAGED =
+      EPI == EPI_BF16R2 && (kSmemBudget - 2048 - 2 * TILE_OUT_BYTES) / STAGE_BYTES >= 4;
+  static constexpr int STAGING_BYTES = STAGED ? (R2_STAGED ? 2 : 1) * TILE_OUT_BYTES : 0;
   static constexpr int NSTAGE_RAW = (kSmemBudget - 2048 - STAGING_BYTES) / STAGE_BYTES;
   static constexpr int NSTAGE = NSTAGE_RAW > 8 ? 8 : NSTAGE_RAW;
   static constexpr int SMEM_BYTES = NSTAGE * STAGE_BYTES + STAGING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
@@ -98,6 +110,12 @@ struct TileWalk {
     }
   }
 };
+
+__device__ __forceinline__ uint32_t lds32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
 
 // m_tile -> tile origin. conv: (w0, h0, img0); linear: (batch index, first row, 0)
 template <bool CONV>
@@ -131,23 +149,32 @@ __device__ __forceinline__ void tile_origin(const GemmEpi& p, int m_tile, int& t
 template <int BN, bool CONV, int EPI>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
-               const __grid_constant__ CUtensorMap mapD, const GemmEpi p, const __grid_constant__ KvMaps kv) {
+               const __grid_constant__ CUtensorMap mapD, const __grid_constant__ CUtensorMap mapR1,
+               const __grid_constant__ CUtensorMap mapR2, const GemmEpi p, const __grid_constant__ KvMaps kv) {
   using C = Cfg<BN, EPI>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
-  uint8_t* staging = smem + C::NSTAGE * C::STAGE_BYTES;
+  uint8_t* staging = smem + C::NSTAGE * C::STAGE_BYTES;  // output tile (and R1), then R2 when C::R2_STAGED
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + C::STAGING_BYTES);
   uint64_t* empty_bar = full_bar + C::NSTAGE;
+  uint64_t* stg_ready = empty_bar + C::NSTAGE;  // staging free for the next tile and its residuals have landed
+  uint64_t* stg_full = stg_ready + 1;           // the consumers have written the tile's output into staging
+  const bool res_staged = (EPI == EPI_BF16 || EPI == EPI_BF16R2) && p.res_tma != 0;  // GEGLU takes no residual
+  const bool r2_staged = C::R2_STAGED && p.res_tma != 0 && p.R2 != nullptr;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&mapA);
     tma_prefetch_desc(&mapB);
     if (C::STAGED) tma_prefetch_desc(&mapD);
+    if (res_staged) tma_prefetch_desc(&mapR1);
+    if (r2_staged) tma_prefetch_desc(&mapR2);
     for (int i = 0; i < C::NSTAGE; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 2);  // one arrival per consumer warpgroup
     }
+    mbar_init(stg_ready, 1);  // the I/O thread (plus the residual bytes)
+    mbar_init(stg_full, 1);   // one consumer thread, after a barrier over all 256
     fence_barrier_init();
   }
   __syncthreads();
@@ -158,6 +185,57 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   if (threadIdx.x < 128) {
     // ------------------------------ TMA producer ------------------------------
     regs_dec<40>();
+    if (C::STAGED && threadIdx.x == 32) {
+      // ---- epilogue I/O: per tile, residuals in, then output out, through the one staging buffer.
+      // Ordering: the residual load of tile t is issued only after bulk_wait_read has seen every TMA store of tile
+      // t-1 finish reading staging (same thread, so its bulk group covers them all), and the consumers touch staging
+      // for tile t only after stg_ready completes for t, i.e. after that load's bytes have arrived (or, without a
+      // staged residual, after the plain arrive that follows the same wait).  The stores of tile t are issued only
+      // after stg_full says both consumer warpgroups wrote it, each thread having fenced its generic-proxy writes
+      // for the async proxy first.  Each barrier is at most one phase ahead of its waiter.
+      uint32_t sphase = 0;
+      const uint32_t stg = smem_u32(staging);
+      TileWalk tw(p);
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, tw.next()) {
+        int t0, t1, t2;
+        tile_origin<CONV>(p, tw.m_tile, t0, t1, t2);
+        const int obase = tw.n_tile * C::OUT_COLS;
+        if (res_staged) {
+          // a tile's residual rows are its own output rows: TMA zero-fills the rows past the end, the store clips them
+          mbar_arrive_expect_tx(stg_ready, C::TILE_OUT_BYTES * (r2_staged ? 2 : 1));
+#pragma unroll 1
+          for (int sub = 0; sub < C::NSUB; ++sub) {
+            uint8_t* dst = staging + sub * C::SUB_BYTES;
+            const int col0 = obase + sub * C::SUBW;
+            if (CONV) tma_load_4d(dst, &mapR1, stg_ready, col0, t0, t1, t2);
+            else tma_load_3d(dst, &mapR1, stg_ready, col0, t1, t0);
+            if (r2_staged) {
+              if (CONV) tma_load_4d(dst + C::TILE_OUT_BYTES, &mapR2, stg_ready, col0, t0, t1, t2);
+              else tma_load_3d(dst + C::TILE_OUT_BYTES, &mapR2, stg_ready, col0, t1, t0);
+            }
+          }
+        } else {
+          mbar_arrive(stg_ready);
+        }
+        mbar_wait(stg_full, sphase);
+        sphase ^= 1u;
+        // the whole bf16 tile is in shared memory: TMA clips it at row / image tails
+#pragma unroll 1
+        for (int sub = 0; sub < C::NSUB; ++sub) {
+          const uint32_t src = stg + static_cast<uint32_t>(sub * C::SUB_BYTES);
+          const int col0 = obase + sub * C::SUBW;
+          if (CONV) tma_store_4d(&mapD, src, col0, t0, t1, t2);
+          else tma_store_3d(&mapD, src, col0, t1, t0);
+          if (!CONV && EPI == EPI_BF16 && kv.n > 0 && col0 >= kv.col0) {
+            // fused all-gather: the same sub-tile into every rank's gather buffer (peer memory over NVLink)
+            for (int i = 0; i < kv.n; ++i) tma_store_3d(&kv.m[i], src, col0 - kv.col0, t1, t0);
+          }
+        }
+        bulk_commit();
+        bulk_wait_read<0>();
+      }
+      bulk_wait_all();  // the last stores have landed before the CTA (and its staging buffer) goes away
+    }
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -234,6 +312,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
   int stage = 0;
   uint32_t phase = 0;
+  uint32_t sphase = 0;
   TileWalk tw(p);
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
     const int n_tile = tw.n_tile;
@@ -267,124 +346,120 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
 
     // ---- epilogue from registers.  acc[4 j + 2 h + e] = tile row tr_base + 8 h, column 8 j + cq + e.
     if (C::STAGED) {
-      // the previous tile's TMA stores must have finished reading the staging buffer
-      if (store_leader) bulk_wait_read<0>();
-      asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory");
+      // the previous tile's TMA stores have finished reading the staging buffer, and this tile's residuals are in it
+      mbar_wait(stg_ready, sphase);
+      sphase ^= 1u;
     }
     const int obase = n_tile * OUT_COLS;  // first output column of this tile
     const int nbase = n_tile * BN;        // first column in the (packed) N space
     // operand pointers at this thread's first column (cq), so that every load of the unrolled column loop below is
     // one instruction with an immediate offset instead of a re-derived address
     const float* bcol = has_bias && EPI != EPI_TRANS ? p.bias + nbase + cq : nullptr;
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int tr = tr_base + 8 * h;
-      long long row = 0;
-      const bool valid = map_row(tr, t0, t1, t2, row);
-      // Rows past the end (tail tiles) read row 0 of the per-frame bias and the residuals instead: their results are
-      // never stored (the TMA store clips them, the fp32 stores check `valid`), and the column loop then branches on
-      // launch-uniform flags only.
-      const long long orow = valid ? row : 0;
-      const float* fb = has_fb ? p.fbias + static_cast<long long>(static_cast<int>(orow) / p.rows_per_frame) * p.ldfb +
-                                     nbase + cq
-                               : nullptr;
-      const bf16* r1p = has_r1 ? p.R1 + orow * p.ldr1 + obase + cq : nullptr;
-      const bf16* r2p = has_r2 ? p.R2 + orow * p.ldr2 + obase + cq : nullptr;
-      float row_bias = 0.f;
-      if (EPI == EPI_TRANS && has_bias && valid) row_bias = __ldg(p.bias + row);
-      const uint32_t swz = SUBW == 32 ? static_cast<uint32_t>((tr >> 1) & 3) : 0u;  // 64B-swizzle XOR of the chunk
-      const uint32_t srow = stg + static_cast<uint32_t>(tr * SUBW * 2 + cq * 2);  // staged row, this thread's column
-#pragma unroll
-      for (int j = 0; j < OUT_COLS / 8; ++j) {
-        const int oc = 8 * j + cq;
-        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-        if (EPI == EPI_TRANS) {
-          v0 += row_bias;
-          v1 += row_bias;
-        } else if (has_bias) {
-          v0 += __ldg(bcol + 8 * j);
-          v1 += __ldg(bcol + 8 * j + 1);
-        }
-        if (has_fb) {
-          v0 += __ldg(fb + 8 * j);
-          v1 += __ldg(fb + 8 * j + 1);
-        }
-        if (GEGLU) {
-          constexpr int JG = BN / 16;  // the gate of column c is column c + BN / 2 of the packed tile
-          float g0 = acc[4 * (j + JG) + 2 * h], g1 = acc[4 * (j + JG) + 2 * h + 1];
-          if (has_bias) {
-            g0 += __ldg(bcol + BN / 2 + 8 * j);
-            g1 += __ldg(bcol + BN / 2 + 8 * j + 1);
-          }
-          v0 *= gelu_erf_fast(g0);
-          v1 *= gelu_erf_fast(g1);
-        } else if (EPI == EPI_F32 && do_silu) {
-          v0 = silu_f(v0);
-          v1 = silu_f(v1);
-        }
-        if (has_r1 || has_r2) {
-          if (has_r1) {
-            const float2 x = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(r1p + 8 * j)));
-            v0 = fmaf(v0, s0, x.x * s1);
-            v1 = fmaf(v1, s0, x.y * s1);
-          } else {
-            v0 *= s0;
-            v1 *= s0;
-          }
-          if (has_r2) {
-            const float2 x = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(r2p + 8 * j)));
-            v0 = fmaf(x.x, s2, v0);
-            v1 = fmaf(x.y, s2, v1);
-          }
-        } else {  // s0 = 1 scales exactly
-          v0 *= s0;
-          v1 *= s0;
-        }
-        if (EPI == EPI_TRANS) {
-          if (valid) {
-            float* dp = static_cast<float*>(p.D) + row;
-            if (obase + oc < p.valid_cols) {
-              float* o = dp + static_cast<long long>(obase + oc) * p.ldd;
-              *o = p.accumulate ? *o + v0 : v0;
-            }
-            if (obase + oc + 1 < p.valid_cols) {
-              float* o = dp + static_cast<long long>(obase + oc + 1) * p.ldd;
-              *o = p.accumulate ? *o + v1 : v1;
-            }
-          }
-        } else if (EPI == EPI_F32) {
-          if (valid)
-            *reinterpret_cast<float2*>(static_cast<float*>(p.D) + row * p.ldd + obase + oc) = make_float2(v0, v1);
-        } else {
-          // sub-tile and 16-byte chunk of column 8 j + cq fold to constants once j is unrolled (cq < 8, SUBW % 8 == 0)
+    // RS: residuals staged in shared memory.  A compile-time flag, so that the unrolled column loop of either form
+    // branches on nothing but the launch-uniform flags above.
+    auto rows = [&](auto staged_tag) {
+      constexpr bool RS = decltype(staged_tag)::value;
+      constexpr bool R2S = RS && C::R2_STAGED;
+  #pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int tr = tr_base + 8 * h;
+        long long row = 0;
+        const bool valid = map_row(tr, t0, t1, t2, row);
+        // Rows past the end (tail tiles) read row 0 of the per-frame bias and of the __ldg residuals instead: their
+        // results are never stored (the TMA store clips them, the fp32 stores check `valid`), and the column loop then
+        // branches on launch-uniform flags only.  Staged residuals read the zeros TMA filled in for those rows.
+        const long long orow = valid ? row : 0;
+        const float* fb = has_fb ? p.fbias + static_cast<long long>(static_cast<int>(orow) / p.rows_per_frame) * p.ldfb +
+                                       nbase + cq
+                                 : nullptr;
+        const bf16* r1p = has_r1 && !RS ? p.R1 + orow * p.ldr1 + obase + cq : nullptr;
+        const bf16* r2p = has_r2 && !R2S ? p.R2 + orow * p.ldr2 + obase + cq : nullptr;
+        float row_bias = 0.f;
+        if (EPI == EPI_TRANS && has_bias && valid) row_bias = __ldg(p.bias + row);
+        const uint32_t swz = SUBW == 32 ? static_cast<uint32_t>((tr >> 1) & 3) : 0u;  // 64B-swizzle XOR of the chunk
+        const uint32_t srow = stg + static_cast<uint32_t>(tr * SUBW * 2 + cq * 2);  // staged row, this thread's column
+  #pragma unroll
+        for (int j = 0; j < OUT_COLS / 8; ++j) {
+          const int oc = 8 * j + cq;
+          // sub-tile and 16-byte chunk of column 8 j + cq fold to constants once j is unrolled (cq < 8, SUBW % 8 == 0);
+          // a staged residual sits at the very address the output goes to
           const int sub = 8 * j / SUBW;
           const int chunk = (8 * j - sub * SUBW) >> 3;
           const uint32_t addr = srow + static_cast<uint32_t>(sub * C::SUB_BYTES) + ((static_cast<uint32_t>(chunk) ^ swz) << 4);
-          asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_bf16x2(v0, v1)) : "memory");
-        }
-      }
-    }
-    if (C::STAGED) {
-      // the whole bf16 tile is in shared memory: one thread hands it to TMA, which clips at row / image tails
-      fence_proxy_async_smem();
-      asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory");
-      if (store_leader) {
-#pragma unroll 1
-        for (int sub = 0; sub < C::NSUB; ++sub) {
-          const uint32_t src = stg + static_cast<uint32_t>(sub * C::SUB_BYTES);
-          const int col0 = obase + sub * SUBW;
-          if (CONV) tma_store_4d(&mapD, src, col0, t0, t1, t2);
-          else tma_store_3d(&mapD, src, col0, t1, t0);
-          if (!CONV && EPI == EPI_BF16 && kv.n > 0 && col0 >= kv.col0) {
-            // fused all-gather: the same sub-tile into every rank's gather buffer (peer memory over NVLink)
-            for (int i = 0; i < kv.n; ++i) tma_store_3d(&kv.m[i], src, col0 - kv.col0, t1, t0);
+          float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+          if (EPI == EPI_TRANS) {
+            v0 += row_bias;
+            v1 += row_bias;
+          } else if (has_bias) {
+            v0 += __ldg(bcol + 8 * j);
+            v1 += __ldg(bcol + 8 * j + 1);
+          }
+          if (has_fb) {
+            v0 += __ldg(fb + 8 * j);
+            v1 += __ldg(fb + 8 * j + 1);
+          }
+          if (GEGLU) {
+            constexpr int JG = BN / 16;  // the gate of column c is column c + BN / 2 of the packed tile
+            float g0 = acc[4 * (j + JG) + 2 * h], g1 = acc[4 * (j + JG) + 2 * h + 1];
+            if (has_bias) {
+              g0 += __ldg(bcol + BN / 2 + 8 * j);
+              g1 += __ldg(bcol + BN / 2 + 8 * j + 1);
+            }
+            v0 *= gelu_erf_fast(g0);
+            v1 *= gelu_erf_fast(g1);
+          } else if (EPI == EPI_F32 && do_silu) {
+            v0 = silu_f(v0);
+            v1 = silu_f(v1);
+          }
+          if (RS || has_r1 || has_r2) {
+            if (RS || has_r1) {
+              const float2 x = unpack_bf16x2(RS ? lds32(addr) : __ldg(reinterpret_cast<const unsigned int*>(r1p + 8 * j)));
+              v0 = fmaf(v0, s0, x.x * s1);
+              v1 = fmaf(v1, s0, x.y * s1);
+            } else {
+              v0 *= s0;
+              v1 *= s0;
+            }
+            if (has_r2) {
+              const float2 x = unpack_bf16x2(R2S ? lds32(addr + C::TILE_OUT_BYTES)
+                                                 : __ldg(reinterpret_cast<const unsigned int*>(r2p + 8 * j)));
+              v0 = fmaf(x.x, s2, v0);
+              v1 = fmaf(x.y, s2, v1);
+            }
+          } else {  // s0 = 1 scales exactly
+            v0 *= s0;
+            v1 *= s0;
+          }
+          if (EPI == EPI_TRANS) {
+            if (valid) {
+              float* dp = static_cast<float*>(p.D) + row;
+              if (obase + oc < p.valid_cols) {
+                float* o = dp + static_cast<long long>(obase + oc) * p.ldd;
+                *o = p.accumulate ? *o + v0 : v0;
+              }
+              if (obase + oc + 1 < p.valid_cols) {
+                float* o = dp + static_cast<long long>(obase + oc + 1) * p.ldd;
+                *o = p.accumulate ? *o + v1 : v1;
+              }
+            }
+          } else if (EPI == EPI_F32) {
+            if (valid)
+              *reinterpret_cast<float2*>(static_cast<float*>(p.D) + row * p.ldd + obase + oc) = make_float2(v0, v1);
+          } else {
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_bf16x2(v0, v1)) : "memory");
           }
         }
-        bulk_commit();
       }
+    };
+    if (res_staged) rows(std::true_type{});
+    else rows(std::false_type{});
+    if (C::STAGED) {
+      // the whole bf16 tile is in shared memory: hand it to the I/O thread, which writes it out by TMA
+      fence_proxy_async_smem();
+      asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory");
+      if (store_leader) mbar_arrive(stg_full);
     }
   }
-  if (C::STAGED && store_leader) bulk_wait_all();  // the staging buffer must outlive the last TMA store reads
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -400,11 +475,16 @@ static int pick_block_n(int N, int act) {
   return 0;
 }
 
+// bf16 output and the residuals staged in its place: one tensor map each, same box and swizzle (zeroed when unused)
+struct OutMaps {
+  CUtensorMap d, r1, r2;
+};
+
 static KvMaps g_kv_none;  // zero-initialised: n = 0
 static const KvMaps* g_kv = &g_kv_none;  // set by v3d_gemm_bf16 around the one launch that scatters K|V
 
 template <int BN, bool CONV, int EPI>
-static int launch(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& md, const GemmEpi& epi,
+static int launch(const CUtensorMap& ma, const CUtensorMap& mb, const OutMaps& mo, const GemmEpi& epi,
                   cudaStream_t st) {
   using C = Cfg<BN, EPI>;
   static bool configured = false;
@@ -419,23 +499,23 @@ static int launch(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMa
   }
   const int total = epi.num_m_tiles * epi.num_n_tiles;
   const int grid = total < num_sms() ? total : num_sms();
-  kern<<<grid, kThreads, C::SMEM_BYTES, st>>>(ma, mb, md, epi, *g_kv);
+  kern<<<grid, kThreads, C::SMEM_BYTES, st>>>(ma, mb, mo.d, mo.r1, mo.r2, epi, *g_kv);
   V3D_CHECK_LAUNCH("gemm_tc_kernel");
   return V3D_OK;
 }
 
 template <int BN, bool CONV>
-static int dispatch_epi(int epi_kind, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& md,
+static int dispatch_epi(int epi_kind, const CUtensorMap& ma, const CUtensorMap& mb, const OutMaps& mo,
                         const GemmEpi& epi, cudaStream_t st) {
   switch (epi_kind) {
-    case EPI_BF16: return launch<BN, CONV, EPI_BF16>(ma, mb, md, epi, st);
-    case EPI_BF16R2: return launch<BN, CONV, EPI_BF16R2>(ma, mb, md, epi, st);
-    case EPI_F32: return launch<BN, CONV, EPI_F32>(ma, mb, md, epi, st);
+    case EPI_BF16: return launch<BN, CONV, EPI_BF16>(ma, mb, mo, epi, st);
+    case EPI_BF16R2: return launch<BN, CONV, EPI_BF16R2>(ma, mb, mo, epi, st);
+    case EPI_F32: return launch<BN, CONV, EPI_F32>(ma, mb, mo, epi, st);
     case EPI_GEGLU:
-      if constexpr (!CONV && (BN / 2) % 16 == 0) return launch<BN, false, EPI_GEGLU>(ma, mb, md, epi, st);
+      if constexpr (!CONV && (BN / 2) % 16 == 0) return launch<BN, false, EPI_GEGLU>(ma, mb, mo, epi, st);
       break;
     case EPI_TRANS:  // at most 128 columns: the per-element transposed stores of wider tiles spill (host caps bn)
-      if constexpr (!CONV && BN <= 128) return launch<BN, false, EPI_TRANS>(ma, mb, md, epi, st);
+      if constexpr (!CONV && BN <= 128) return launch<BN, false, EPI_TRANS>(ma, mb, mo, epi, st);
       break;
   }
   set_error("unsupported epilogue %d for this mode/tile", epi_kind);
@@ -443,15 +523,15 @@ static int dispatch_epi(int epi_kind, const CUtensorMap& ma, const CUtensorMap& 
 }
 
 template <bool CONV>
-static int dispatch_bn(int bn, int epi_kind, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& md,
+static int dispatch_bn(int bn, int epi_kind, const CUtensorMap& ma, const CUtensorMap& mb, const OutMaps& mo,
                        const GemmEpi& epi, cudaStream_t st) {
   switch (bn) {
-    case 256: return dispatch_epi<256, CONV>(epi_kind, ma, mb, md, epi, st);
-    case 160: return dispatch_epi<160, CONV>(epi_kind, ma, mb, md, epi, st);
-    case 128: return dispatch_epi<128, CONV>(epi_kind, ma, mb, md, epi, st);
-    case 64: return dispatch_epi<64, CONV>(epi_kind, ma, mb, md, epi, st);
-    case 32: return dispatch_epi<32, CONV>(epi_kind, ma, mb, md, epi, st);
-    case 16: return dispatch_epi<16, CONV>(epi_kind, ma, mb, md, epi, st);
+    case 256: return dispatch_epi<256, CONV>(epi_kind, ma, mb, mo, epi, st);
+    case 160: return dispatch_epi<160, CONV>(epi_kind, ma, mb, mo, epi, st);
+    case 128: return dispatch_epi<128, CONV>(epi_kind, ma, mb, mo, epi, st);
+    case 64: return dispatch_epi<64, CONV>(epi_kind, ma, mb, mo, epi, st);
+    case 32: return dispatch_epi<32, CONV>(epi_kind, ma, mb, mo, epi, st);
+    case 16: return dispatch_epi<16, CONV>(epi_kind, ma, mb, mo, epi, st);
     default: set_error("unsupported block_n %d", bn); return V3D_ERR_BAD_ARG;
   }
 }
@@ -513,9 +593,16 @@ extern "C" int v3d_gemm_bf16(const v3d_gemm_args* a, void* stream) {
     set_error("v3d_gemm_bf16: ntaps must be 1 or 3");
     return V3D_ERR_BAD_ARG;
   }
-  if ((a->lda % 8) || (a->ldb % 8) || (a->ldd % 8) || (a->R1 && a->ldr1 % 8) || (a->R2 && a->ldr2 % 8) ||
-      (a->ldfb % 4)) {
+  if ((a->lda % 8) || (a->ldb % 8) || (a->ldd % 8) || (a->ldfb % 4)) {
     set_error("v3d_gemm_bf16: leading dimensions must be multiples of 8 elements");
+    return V3D_ERR_BAD_ARG;
+  }
+  // the epilogue reads residuals two columns at a time (4 bytes); TMA staging needs 16-byte alignment on top
+  auto res_ok = [](const void* r, int64_t ld) { return r == nullptr || (ld % 2 == 0 && (reinterpret_cast<uintptr_t>(r) & 3) == 0); };
+  auto res_tma = [](const void* r, int64_t ld) { return r != nullptr && ld % 8 == 0 && (reinterpret_cast<uintptr_t>(r) & 15) == 0; };
+  if (!res_ok(a->R1, a->ldr1) || !res_ok(a->R2, a->ldr2)) {
+    set_error("v3d_gemm_bf16: residuals need an even row pitch and a 4-byte aligned base (ldr1=%lld ldr2=%lld)",
+              static_cast<long long>(a->ldr1), static_cast<long long>(a->ldr2));
     return V3D_ERR_BAD_ARG;
   }
   int bn = a->block_n > 0 ? a->block_n : pick_block_n(a->N, a->act);
@@ -680,8 +767,8 @@ extern "C" int v3d_gemm_bf16(const v3d_gemm_args* a, void* stream) {
     set_error("v3d_gemm_bf16: act=%d is not available with this output mode", a->act);
     return V3D_ERR_UNSUPPORTED;
   }
-  CUtensorMap md;
-  memset(&md, 0, sizeof(md));
+  OutMaps mo;
+  memset(&mo, 0, sizeof(mo));
   if (e.R2 != nullptr && e.R1 == nullptr) {  // a lone residual always travels as R1
     e.R1 = e.R2; e.ldr1 = e.ldr2; e.s1 = e.s2;
     e.R2 = nullptr;
@@ -692,18 +779,33 @@ extern "C" int v3d_gemm_bf16(const v3d_gemm_args* a, void* stream) {
     const uint32_t ocols_tile = epi_kind == EPI_GEGLU ? bn / 2 : bn;
     const uint32_t subw = ocols_tile % 32 == 0 ? 32 : 16;  // must match SUBW in the kernel
     const int swz = subw == 32 ? 64 : 0;
-    if (conv) {
-      const uint64_t dims[4] = {out_cols, (uint64_t)e.cw, (uint64_t)e.ch, (uint64_t)e.cn};
-      const uint64_t str[3] = {(uint64_t)a->ldd * 2, (uint64_t)a->ldd * 2 * e.cw, (uint64_t)a->ldd * 2 * e.cw * e.ch};
-      const uint32_t box[4] = {subw, (uint32_t)e.bw, (uint32_t)e.bh, (uint32_t)e.bn};
-      rc = make_tmap_bf16(&md, a->D, 4, dims, str, box, swz);
-    } else {
+    // the output's tile boxes over a matrix of pitch ld: the output itself, and the residuals, whose rows are the
+    // output rows in every mode (a temporal GEMM's residual is not tap-shifted)
+    auto out_map = [&](CUtensorMap* m, const void* base, long long ld) {
+      if (conv) {
+        const uint64_t dims[4] = {out_cols, (uint64_t)e.cw, (uint64_t)e.ch, (uint64_t)e.cn};
+        const uint64_t str[3] = {(uint64_t)ld * 2, (uint64_t)ld * 2 * e.cw, (uint64_t)ld * 2 * e.cw * e.ch};
+        const uint32_t box[4] = {subw, (uint32_t)e.bw, (uint32_t)e.bh, (uint32_t)e.bn};
+        return make_tmap_bf16(m, base, 4, dims, str, box, swz);
+      }
       const uint64_t dims[3] = {out_cols, (uint64_t)e.rows_per_batch, (uint64_t)e.batch};
-      const uint64_t str[2] = {(uint64_t)a->ldd * 2, (uint64_t)a->ldd * 2 * e.rows_per_batch};
+      const uint64_t str[2] = {(uint64_t)ld * 2, (uint64_t)ld * 2 * e.rows_per_batch};
       const uint32_t box[3] = {subw, BM, 1};
-      rc = make_tmap_bf16(&md, a->D, 3, dims, str, box, swz);
-    }
+      return make_tmap_bf16(m, base, 3, dims, str, box, swz);
+    };
+    rc = out_map(&mo.d, a->D, a->ldd);
     if (rc) return rc;
+    // residuals are staged only if TMA can address all of them (16-byte aligned bases and pitches); otherwise the
+    // epilogue reads them with __ldg
+    if (res_tma(e.R1, e.ldr1) && (e.R2 == nullptr || res_tma(e.R2, e.ldr2))) {
+      e.res_tma = 1;
+      rc = out_map(&mo.r1, e.R1, e.ldr1);
+      if (rc) return rc;
+      if (e.R2 != nullptr) {
+        rc = out_map(&mo.r2, e.R2, e.ldr2);
+        if (rc) return rc;
+      }
+    }
   }
   // fused GEMM -> all-gather (K|V scatter into peer memory): plain linear bf16-output launches only
   KvMaps kvm;
@@ -730,7 +832,7 @@ extern "C" int v3d_gemm_bf16(const v3d_gemm_args* a, void* stream) {
     }
     g_kv = &kvm;
   }
-  rc = conv ? dispatch_bn<true>(bn, epi_kind, ma, mb, md, e, st) : dispatch_bn<false>(bn, epi_kind, ma, mb, md, e, st);
+  rc = conv ? dispatch_bn<true>(bn, epi_kind, ma, mb, mo, e, st) : dispatch_bn<false>(bn, epi_kind, ma, mb, mo, e, st);
   g_kv = &g_kv_none;
   return rc;
 }

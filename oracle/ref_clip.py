@@ -96,28 +96,48 @@ def preprocess(x: torch.Tensor, size: int = 224) -> torch.Tensor:
     return (x - mean) / std
 
 
-def clip_visual_forward(sd: SD, spec: ClipSpec, img: torch.Tensor) -> torch.Tensor:
-    """open_clip VisionTransformer.forward on preprocessed images [B, 3, 224, 224] -> pooled embedding [B, embed_dim]"""
-    B = img.shape[0]
-    w, hd = spec.width, spec.width // spec.heads
+def clip_embed(sd: SD, spec: ClipSpec, img: torch.Tensor) -> torch.Tensor:
+    """conv1 patches, [class_embedding; patches] + positional_embedding, ln_pre -> residual stream [B, n, width]"""
+    B, w = img.shape[0], spec.width
     x = F.conv2d(img, sd["conv1.weight"], None, stride=spec.patch)            # [B, w, g, g]
     x = x.reshape(B, w, -1).permute(0, 2, 1)                                  # [B, g*g, w]
     x = torch.cat([sd["class_embedding"].to(x).expand(B, 1, w), x], dim=1) + sd["positional_embedding"]
-    x = F.layer_norm(x, (w,), sd["ln_pre.weight"], sd["ln_pre.bias"], 1e-5)
-    n = x.shape[1]
-    for i in range(spec.layers):
-        p = f"transformer.resblocks.{i}."
-        h = F.layer_norm(x, (w,), sd[p + "ln_1.weight"], sd[p + "ln_1.bias"], 1e-5)
-        qkv = F.linear(h, sd[p + "attn.in_proj_weight"], sd[p + "attn.in_proj_bias"])
-        q, k, v = [t.reshape(B, n, spec.heads, hd).permute(0, 2, 1, 3) for t in qkv.chunk(3, dim=-1)]
-        att = torch.softmax(q @ k.transpose(-1, -2) / math.sqrt(hd), dim=-1) @ v
-        att = att.permute(0, 2, 1, 3).reshape(B, n, w)
-        x = x + F.linear(att, sd[p + "attn.out_proj.weight"], sd[p + "attn.out_proj.bias"])
-        h = F.layer_norm(x, (w,), sd[p + "ln_2.weight"], sd[p + "ln_2.bias"], 1e-5)
-        h = F.gelu(F.linear(h, sd[p + "mlp.c_fc.weight"], sd[p + "mlp.c_fc.bias"]))
-        x = x + F.linear(h, sd[p + "mlp.c_proj.weight"], sd[p + "mlp.c_proj.bias"])
-    pooled = F.layer_norm(x[:, 0], (w,), sd["ln_post.weight"], sd["ln_post.bias"], 1e-5)
+    return F.layer_norm(x, (w,), sd["ln_pre.weight"], sd["ln_pre.bias"], 1e-5)
+
+
+def clip_attn_half(sd: SD, spec: ClipSpec, i: int, x: torch.Tensor) -> torch.Tensor:
+    """x + out_proj(MHA(ln_1(x))) of residual block i (16 heads of width 80 at ViT-H/14)"""
+    B, n, w = x.shape
+    hd = w // spec.heads
+    p = f"transformer.resblocks.{i}."
+    h = F.layer_norm(x, (w,), sd[p + "ln_1.weight"], sd[p + "ln_1.bias"], 1e-5)
+    qkv = F.linear(h, sd[p + "attn.in_proj_weight"], sd[p + "attn.in_proj_bias"])
+    q, k, v = [t.reshape(B, n, spec.heads, hd).permute(0, 2, 1, 3) for t in qkv.chunk(3, dim=-1)]
+    att = torch.softmax(q @ k.transpose(-1, -2) / math.sqrt(hd), dim=-1) @ v
+    att = att.permute(0, 2, 1, 3).reshape(B, n, w)
+    return x + F.linear(att, sd[p + "attn.out_proj.weight"], sd[p + "attn.out_proj.bias"])
+
+
+def clip_mlp_half(sd: SD, spec: ClipSpec, i: int, x: torch.Tensor) -> torch.Tensor:
+    """x + c_proj(gelu_erf(c_fc(ln_2(x)))) of residual block i"""
+    p = f"transformer.resblocks.{i}."
+    h = F.layer_norm(x, (spec.width,), sd[p + "ln_2.weight"], sd[p + "ln_2.bias"], 1e-5)
+    h = F.gelu(F.linear(h, sd[p + "mlp.c_fc.weight"], sd[p + "mlp.c_fc.bias"]))
+    return x + F.linear(h, sd[p + "mlp.c_proj.weight"], sd[p + "mlp.c_proj.bias"])
+
+
+def clip_head(sd: SD, spec: ClipSpec, x: torch.Tensor) -> torch.Tensor:
+    """ln_post on the class token, @ proj -> pooled embedding [B, embed_dim]"""
+    pooled = F.layer_norm(x[:, 0], (spec.width,), sd["ln_post.weight"], sd["ln_post.bias"], 1e-5)
     return pooled @ sd["proj"]
+
+
+def clip_visual_forward(sd: SD, spec: ClipSpec, img: torch.Tensor) -> torch.Tensor:
+    """open_clip VisionTransformer.forward on preprocessed images [B, 3, 224, 224] -> pooled embedding [B, embed_dim]"""
+    x = clip_embed(sd, spec, img)
+    for i in range(spec.layers):
+        x = clip_mlp_half(sd, spec, i, clip_attn_half(sd, spec, i, x))
+    return clip_head(sd, spec, x)
 
 
 def image_embedder_forward(sd: SD, spec: ClipSpec, image: torch.Tensor, n_cond_frames: int = 1,

@@ -74,6 +74,22 @@ def attn_block(sd: SD, p: str, x):
     return x + F.conv2d(o, sd[p + ".proj_out.weight"], sd[p + ".proj_out.bias"])
 
 
+def upsample(sd: SD, p: str, x):
+    """Upsample (model.py:60-71): nearest 2x, then the 3x3 conv `p`."""
+    return F.conv2d(F.interpolate(x, scale_factor=2.0, mode="nearest"), sd[p + ".weight"], sd[p + ".bias"], padding=1)
+
+
+def decoder_tail(sd: SD, h, T: int):
+    """norm_out -> swish -> conv_out, then AE3DConv's time_mix_conv (temporal_ae.py:101-107): a (3, 1, 1) conv over
+    each clip of T frames, zero-padded at the clip's two ends."""
+    h = _swish(_norm(h, sd, "norm_out"))
+    h = F.conv2d(h, sd["conv_out.weight"], sd["conv_out.bias"], padding=1)
+    bt, c, hh, ww = h.shape
+    h5 = h.reshape(bt // T, T, c, hh, ww).permute(0, 2, 1, 3, 4)
+    h5 = F.conv3d(h5, sd["conv_out.time_mix_conv.weight"], sd["conv_out.time_mix_conv.bias"], padding=(1, 0, 0))
+    return h5.permute(0, 2, 1, 3, 4).reshape(bt, c, hh, ww)
+
+
 def decoder_forward(sd: SD, spec: DecoderSpec, z, T: int, taps=None):
     """Decoder.forward (model.py:715-748) with AE3DConv.forward at the end (temporal_ae.py:101-107)."""
     nres = len(spec.ch_mult)
@@ -87,16 +103,10 @@ def decoder_forward(sd: SD, spec: DecoderSpec, z, T: int, taps=None):
         for j in range(spec.num_res_blocks + 1):
             h = video_res_block(sd, f"up.{lvl}.block.{j}", h, T)
         if lvl != 0:
-            h = F.interpolate(h, scale_factor=2.0, mode="nearest")  # Upsample, model.py:67-71
-            h = F.conv2d(h, sd[f"up.{lvl}.upsample.conv.weight"], sd[f"up.{lvl}.upsample.conv.bias"], padding=1)
+            h = upsample(sd, f"up.{lvl}.upsample.conv", h)
         if taps is not None:
             taps[f"up.{lvl}"] = h
-    h = _swish(_norm(h, sd, "norm_out"))
-    h = F.conv2d(h, sd["conv_out.weight"], sd["conv_out.bias"], padding=1)
-    bt, c, hh, ww = h.shape
-    h5 = h.reshape(bt // T, T, c, hh, ww).permute(0, 2, 1, 3, 4)
-    h5 = F.conv3d(h5, sd["conv_out.time_mix_conv.weight"], sd["conv_out.time_mix_conv.bias"], padding=(1, 0, 0))
-    return h5.permute(0, 2, 1, 3, 4).reshape(bt, c, hh, ww)
+    return decoder_tail(sd, h, T)
 
 
 def decode_first_stage(sd: SD, spec: DecoderSpec, z, n_samples_a_time: int, scale_factor: float = 0.18215):

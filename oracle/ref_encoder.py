@@ -30,6 +30,16 @@ class EncoderSpec:
     double_z: bool = True
 
 
+def downsample(sd: SD, p: str, x: torch.Tensor) -> torch.Tensor:
+    """Downsample (model.py:74-91): zero padding on the bottom / right only, then the stride-2 3x3 conv `p`."""
+    return F.conv2d(F.pad(x, (0, 1, 0, 1), mode="constant", value=0), sd[p + ".weight"], sd[p + ".bias"], stride=2)
+
+
+def encoder_tail(sd: SD, h: torch.Tensor) -> torch.Tensor:
+    """norm_out -> swish -> conv_out: the moments [B, 2z, H/8, W/8]"""
+    return F.conv2d(_swish(_norm(h, sd, "norm_out")), sd["conv_out.weight"], sd["conv_out.bias"], padding=1)
+
+
 def encoder_forward(sd: SD, spec: EncoderSpec, x: torch.Tensor) -> torch.Tensor:
     """Encoder.forward with temb = None: conv_in, per level num_res_blocks ResnetBlocks (+ asymmetric-pad stride-2
     conv between levels, model.py:74-91), mid block/attn/block, GroupNorm + swish + conv_out -> [B, 2z, H/8, W/8]."""
@@ -39,13 +49,11 @@ def encoder_forward(sd: SD, spec: EncoderSpec, x: torch.Tensor) -> torch.Tensor:
         for blk in range(spec.num_res_blocks):
             h = resnet_block(sd, f"down.{lvl}.block.{blk}", h)
         if lvl != nres - 1:
-            h = F.pad(h, (0, 1, 0, 1), mode="constant", value=0)
-            h = F.conv2d(h, sd[f"down.{lvl}.downsample.conv.weight"], sd[f"down.{lvl}.downsample.conv.bias"], stride=2)
+            h = downsample(sd, f"down.{lvl}.downsample.conv", h)
     h = resnet_block(sd, "mid.block_1", h)
     h = attn_block(sd, "mid.attn_1", h)
     h = resnet_block(sd, "mid.block_2", h)
-    h = _swish(_norm(h, sd, "norm_out"))
-    return F.conv2d(h, sd["conv_out.weight"], sd["conv_out.bias"], padding=1)
+    return encoder_tail(sd, h)
 
 
 def gaussian_sample(moments: torch.Tensor, noise: torch.Tensor) -> torch.Tensor:

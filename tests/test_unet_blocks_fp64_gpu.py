@@ -57,7 +57,7 @@ import torch.nn.functional as F
 
 sys.path.insert(0, str(Path(__file__).resolve().parent))
 
-from framewise import assert_per_sample  # noqa: E402
+from framewise import LOCALITY_FACTOR, LOCALITY_FLOOR, assert_per_sample, groups, judge, ring_interior  # noqa: E402
 
 GOLD = Path(__file__).resolve().parent / "golden"
 PERFRAME = json.loads((GOLD / "PERFRAME.json").read_text())
@@ -74,7 +74,6 @@ STANDIN_MARGIN = 1.25
 STANDIN_C = {"conv_in": 7.07e-4, "res": 7.16e-3, "res_skip": 1.85e-3, "attn": 4.26e-3, "down": 7.28e-4,
              "up": 7.07e-4, "out": 2.24e-3}
 C_KIND = {k: STANDIN_MARGIN * v for k, v in STANDIN_C.items()}
-LOCALITY_FACTOR, LOCALITY_FLOOR = 2.0, 0.1
 
 # leg -> (model_channels, T, latent, weight seed); the fixture legs take their inputs from make_golden_perframe
 GPU_LEGS = {"unet_small_t18_perframe": None, "unet_full_t5_perframe": None, "bench_v3d512": (320, 18, 64, 3)}
@@ -121,46 +120,20 @@ def _kind(kind, prm):
     return "res_skip" if kind == "res" and prm["cin"] != prm["cout"] else kind
 
 
-def judge(name, kind, x_in, ref, got, T, c, bf16_out=True):
-    """Budget and locality of one block; returns a record, prints the BLOCK line."""
-    err = got - ref
-    upd = ref - x_in if x_in.shape == ref.shape else ref
-    rnd = ref.to(torch.bfloat16).to(ref.dtype) - ref if bf16_out else torch.zeros_like(ref)
-    S = torch.stack([err.square(), upd.square(), rnd.square()])               # [3, B, C, H, W]
-    del err, upd, rnd
-    B, C, H, W = ref.shape
-    bc = S.sum((3, 4))                                                        # [3, B, C]
-    tot = bc.sum((1, 2))
-
-    def ratio(s):                                                             # s: [3, ...] sums of squares
-        s = s.sqrt()
-        return s[0] / (c * s[1] + s[2]).clamp_min(1e-300)
-
-    whole = float(ratio(tot))
-    sample = bc.sum(2)
-    g = min(32, C)
-    parts = {"sample": sample, "frame": sample.reshape(3, B // T, T).sum(1),
-             "chan32": bc.sum(1).reshape(3, C // g, g).sum(2)}
-    if kind == "attn":
-        parts["head"] = bc.sum(1).reshape(3, C // 64, 64).sum(2)
-    if H >= 8 and W >= 8:
-        ring = S.sum((1, 2))
-        ring[:, 1:-1, 1:-1] = 0
-        ring = ring.sum((1, 2))
-        parts["ring|interior"] = torch.stack([ring, tot - ring], 1)
-    worst, local_bad = ("whole", 0, whole), []
-    limit = LOCALITY_FACTOR * whole + LOCALITY_FLOOR
-    for pname, s in parts.items():
-        r = ratio(s).cpu()
-        i = int(r.argmax())
-        if float(r[i]) > worst[2]:
-            worst = (pname, i, float(r[i]))
-        local_bad += [(pname, j, round(float(r[j]), 3)) for j in range(r.numel()) if float(r[j]) > limit]
-    s = tot.sqrt()
-    c_meas = float((s[0] - s[2]).clamp_min(0.0) / s[1].clamp_min(1e-300))
-    print(f"BLOCK {name} kind={kind} ratio={whole:.3f} worst={worst[0]}:{worst[1]}:{worst[2]:.3f} c={c_meas:.3e}")
-    return dict(name=name, kind=kind, ratio=whole, worst=worst, c=c_meas, local_bad=local_bad,
-                finite=bool(torch.isfinite(got).all()))
+def unet_parts(kind, T):
+    """The UNet's partitions of a block output [B, C, H, W]: each of the 2T samples, each frame position t, each
+    32-channel group, each 64-channel head (attention blocks), the border ring vs the interior (h, w >= 8)."""
+    def parts(sq):
+        B, C, H, W = sq.shape
+        bc = sq.sum((2, 3))
+        sample = bc.sum(1)
+        p = {"sample": sample, "frame": sample.reshape(B // T, T).sum(0), "chan32": groups(bc.sum(0), min(32, C))}
+        if kind == "attn":
+            p["head"] = groups(bc.sum(0), 64)
+        if H >= 8 and W >= 8:
+            p["ring|interior"] = ring_interior(sq.sum((0, 1)))
+        return p
+    return parts
 
 
 @torch.no_grad()
@@ -200,7 +173,7 @@ def check_blocks(sd, spec, xin, ts, ctx, y, T, out, taps, dev, c_kind=None):
                            sd["out.2.bias"], padding=1)
         got = (out if kind == "out" else taps[name]).to(dev, f64)
         k = _kind(kind, prm)
-        rows.append(judge(name, k, cur, ref, got, T, c_kind[k], bf16_out=kind != "out"))
+        rows.append(judge(name, k, cur, ref, got, c_kind[k], unet_parts(k, T), bf16_out=kind != "out"))
         cur = got
         if kind == "conv_in":
             hs.append(cur)
@@ -259,11 +232,11 @@ def test_block_check_flags_a_wrong_frame():
     x_in = torch.randn(B, C, H, H, generator=g, dtype=torch.float64)
     ref = x_in + 0.3 * torch.randn(B, C, H, H, generator=g, dtype=torch.float64)
     good = ref.to(torch.bfloat16).double()
-    r = judge("synthetic", "res", x_in, ref, good, T, 1e-3)
+    r = judge("synthetic", "res", x_in, ref, good, 1e-3, unet_parts("res", T))
     assert r["ratio"] <= 1.0 and not r["local_bad"], r
     bad = good.clone()
     bad[T - 1] = good[T - 2]                              # the last frame of the first video reads its neighbour
-    r = judge("synthetic", "res", x_in, ref, bad, T, 1e-3)
+    r = judge("synthetic", "res", x_in, ref, bad, 1e-3, unet_parts("res", T))
     assert r["ratio"] > 1.0 and r["worst"][0] in ("sample", "frame") and r["worst"][1] == T - 1, r
     assert ("sample", T - 1) in [p[:2] for p in r["local_bad"]], r
 

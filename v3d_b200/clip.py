@@ -99,6 +99,9 @@ class FrozenOpenCLIPImageEmbedder(KernelModule):
         self.antialias, self.ucg_rate, self.unsqueeze_dim, self.max_length = antialias, ucg_rate, unsqueeze_dim, max_length
         self.register_buffer("mean", torch.tensor(CLIP_MEAN), persistent=False)
         self.register_buffer("std", torch.tensor(CLIP_STD), persistent=False)
+        # tests: {name: None} -> filled with the fp32 residual stream [B, n, width] after ln_pre ("pre") and after the
+        # attention / MLP half of layer i ("L{i}.attn", "L{i}.mlp")
+        self.debug_taps: Optional[dict] = None
 
     def freeze(self):
         self.eval()
@@ -149,6 +152,10 @@ class FrozenOpenCLIPImageEmbedder(KernelModule):
         return P
 
     # ---- the tower ---------------------------------------------------------------------------------------------------
+    def _tap(self, name: str, x: torch.Tensor, B: int, n: int) -> None:
+        if self.debug_taps is not None and name in self.debug_taps:
+            self.debug_taps[name] = x.view(B, n, -1).float()     # exactly what the next half reads
+
     @torch.no_grad()
     def encode_with_vision_transformer(self, img: torch.Tensor) -> torch.Tensor:
         ops.require_current_device(img, "v3d_b200.FrozenOpenCLIPImageEmbedder")
@@ -172,11 +179,12 @@ class FrozenOpenCLIPImageEmbedder(KernelModule):
         xb = torch.empty_like(xa)
         ops.layernorm(xa, xb, *P["ln_pre"], rows, w)
         x_res = xb                                                           # residual stream, bf16 [rows, w]
+        self._tap("pre", x_res, B, n)
         hp = (hd + 63) // 64 * 64                                            # head width padded for the contraction
         nk = (n + 63) // 64 * 64                                             # keys padded for the P V contraction
         h_ln = torch.empty_like(x_res)
         qkv = torch.empty(rows, 3 * w, device=dev, dtype=bf16)
-        for blk in P["blocks"]:
+        for i, blk in enumerate(P["blocks"]):
             ops.layernorm(x_res, h_ln, *blk["ln1"], rows, w)
             ops.gemm(h_ln, blk["qkv_w"], qkv, K=w, N=3 * w, rows_per_batch=rows, bias=blk["qkv_b"])
             q, k, val = [t.reshape(B, n, heads, hd).permute(0, 2, 1, 3) for t in qkv.view(B, n, 3 * w).split(w, dim=-1)]
@@ -198,11 +206,13 @@ class FrozenOpenCLIPImageEmbedder(KernelModule):
             att = o.view(B, heads, n, hd).permute(0, 2, 1, 3).reshape(rows, w).contiguous()
             x_new = torch.empty_like(x_res)
             ops.gemm(att, blk["out_w"], x_new, K=w, N=w, rows_per_batch=rows, bias=blk["out_b"], r1=x_res, s1=1.0)
+            self._tap(f"L{i}.attn", x_new, B, n)
             ops.layernorm(x_new, h_ln, *blk["ln2"], rows, w)
             m = torch.empty(rows, v.mlp, device=dev, dtype=bf16)
             ops.gemm(h_ln, blk["fc_w"], m, K=w, N=2 * v.mlp, rows_per_batch=rows, bias=blk["fc_b"], act=ops.ACT_GEGLU)
             x_res = torch.empty_like(x_new)
             ops.gemm(m, blk["proj_w"], x_res, K=v.mlp, N=w, rows_per_batch=rows, bias=blk["proj_b"], r1=x_new, s1=1.0)
+            self._tap(f"L{i}.mlp", x_res, B, n)
         cls = x_res.view(B, n, w)[:, 0].contiguous()
         pooled = torch.empty_like(cls)
         ops.layernorm(cls, pooled, *P["ln_post"], B, w)

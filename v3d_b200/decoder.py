@@ -74,6 +74,7 @@ class VideoDecoder(KernelModule):
         self.merge_strategy = merge_strategy
         self.time_mode = time_mode
         self.num_resolutions = len(self.ch_mult)
+        self.debug_taps: Optional[dict] = None  # tests: {block name: None} -> filled with NCHW fp32 outputs
         for key, shape in self.param_shapes().items():
             _register(self, key, self._init_value(key, shape))
 
@@ -264,6 +265,14 @@ class VideoDecoder(KernelModule):
                  b_batch_stride=hw, bias=P[key + ".v.bias"])
         return self._linear(P, key + ".proj_out", o, rows, out=xn, r1=x, s1=1.0)
 
+    def _tap(self, name, x, B, c, h, w):
+        """With `debug_taps` holding `name`: the block output x (bf16 NHWC) widened to fp32 NCHW, which is exactly
+        the next block's input.  Launches nothing when taps are off."""
+        if self.debug_taps is not None and name in self.debug_taps:
+            tap = torch.empty(B, c, h, w, device=x.device, dtype=torch.float32)
+            ops.nhwc_to_nchw_f32(x, tap, B, c, h * w, c)
+            self.debug_taps[name] = tap
+
     def forward(self, z: torch.Tensor, timesteps: Optional[int] = None, skip_video: bool = False, **kwargs):
         if skip_video:
             raise NotImplementedError("skip_video decode is not implemented")
@@ -284,6 +293,8 @@ class VideoDecoder(KernelModule):
         """The launch schedule of one decode (Decoder.forward, model.py:715-748, through VideoDecoder)."""
         vs = self.view_shard
         if vs is not None:
+            if self.debug_taps is not None:
+                raise NotImplementedError("debug_taps are not supported by the frame-sharded decode")
             vs.begin("decoder")
         dev, zc = z.device, self.z_channels
         n_norms = 4 * sum(1 for n, _, _ in self._blocks() if not n.startswith("@")) + 2
@@ -294,6 +305,7 @@ class VideoDecoder(KernelModule):
             h, w = H, W
             cur = self._conv3x3(P, "conv_in", cur, B, h, w, zc)
             ch = self.ch * self.ch_mult[-1]
+            self._tap("conv_in", cur, B, ch, h, w)
             for name, ci, co in self._blocks():
                 if name.startswith("@attn:"):
                     if (h * w) % 64 != 0 or ci % 64 != 0:
@@ -308,6 +320,7 @@ class VideoDecoder(KernelModule):
                 else:
                     cur = self._video_res_block(P, name, ci, co, cur, B, T, nb, h, w)
                     ch = co
+                self._tap(name.rsplit(":", 1)[-1], cur, B, ch, h, w)
             a = self._gn(P, "norm_out", cur, h * w, B, ch, 1e-6, True)
             if vs is None:
                 o = self._conv3x3(P, "conv_out", a, B, h, w, ch, out_dtype=torch.float32)   # [rows, 16] fp32

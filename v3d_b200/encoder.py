@@ -60,6 +60,7 @@ class Encoder(KernelModule):
         self.resolution = resolution
         self.num_resolutions = len(self.ch_mult)
         self.out_channels = (2 if double_z else 1) * z_channels
+        self.debug_taps: Optional[dict] = None  # tests: {block name: None} -> filled with NCHW fp32 outputs
         for key, shape in self.param_shapes().items():
             _register(self, key, self._init_value(key, shape))
 
@@ -168,6 +169,7 @@ class Encoder(KernelModule):
 
     # --------------------------------------------------------------------------------------------
     _attn = VideoDecoder._attn  # AttnBlock (model.py:161-201): same single-head block as the decoder's mid.attn_1
+    _tap = VideoDecoder._tap
 
     def _res_block(self, P, name, ci, co, x, B, h, w):
         """ResnetBlock.forward with temb = None (model.py:131-151)."""
@@ -210,6 +212,7 @@ class Encoder(KernelModule):
             h, w = H, W
             cur = self._conv3x3(P, "conv_in", cur, B, h, w, cin)
             ch = self.ch
+            self._tap("conv_in", cur, B, ch, h, w)
             for name, ci, co in self._blocks():
                 if name.startswith("@attn:"):
                     if (h * w) % 64 != 0 or ci % 64 != 0:
@@ -220,6 +223,7 @@ class Encoder(KernelModule):
                 else:
                     cur = self._res_block(P, name, ci, co, cur, B, h, w)
                     ch = co
+                self._tap(name.rsplit(":", 1)[-1], cur, B, ch, h, w)
             a = self._gn(P, "norm_out", cur, h * w, B, ch, 1e-6, True)
             o = self._conv3x3(P, "conv_out", a, B, h, w, ch, out_dtype=torch.float32)   # [rows, 16] fp32
             out = torch.empty(B, self.out_channels, h, w, device=dev, dtype=torch.float32)

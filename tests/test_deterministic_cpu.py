@@ -16,7 +16,7 @@ import torch
 ROOT = str(Path(__file__).resolve().parent.parent)
 sys.path.insert(0, str(Path(__file__).resolve().parent))
 
-from test_host_schedule_cpu import _build_decoder, _build_unet, _cos, _rel, _unet, _unet_inputs  # noqa: E402
+from test_host_schedule_cpu import LAUNCHES, _build_decoder, _build_unet, _cos, _rel, _unet, _unet_inputs  # noqa: E402
 
 NEW_SYMBOLS = ["v3d_groupnorm_det_blocks", "v3d_groupnorm_det_workspace_bytes", "v3d_groupnorm_partials",
                "v3d_groupnorm_fold_apply", "v3d_groupnorm_det"]
@@ -134,23 +134,27 @@ def test_det_unet_and_decoder_schedules_match_oracle(det_mode):
     T, hw = 3, 16
     net, sd = _build_unet()
     xin, ts, ctx, y = _unet_inputs(T, hw)
-    with emu_ops.patched():
+    calls = []
+    with emu_ops.patched(calls):
         out = _unet(net, xin, ts, ctx, y, T)
     with torch.no_grad():
         ref = ref_unet.unet_forward(sd, ref_unet.UNetSpec(model_channels=64), xin, ts, ctx, y, T, torch.zeros(2, T))
     r, cs = _rel(out, ref), _cos(out, ref)
-    print("det unet schedule vs oracle: rel-L2", r, "cos", cs)
+    print("det unet schedule vs oracle: rel-L2", r, "cos", cs, "launches", emu_ops.digest(calls))
     assert r <= 3e-2 and cs >= 0.999, (r, cs)
+    assert emu_ops.digest(calls) == LAUNCHES["unet_t3_deterministic"]
 
     dec, sdd = _build_decoder()
     z = torch.randn(T, 4, 8, 8, generator=torch.Generator().manual_seed(3))
-    with emu_ops.patched():
+    calls = []
+    with emu_ops.patched(calls):
         out = dec(z, timesteps=T)
     with torch.no_grad():
         ref = ref_decoder.decoder_forward(sdd, ref_decoder.DecoderSpec(ch=64), z, T)
     r, cs = _rel(out, ref), _cos(out, ref)
-    print("det decoder schedule vs oracle: rel-L2", r, "cos", cs)
+    print("det decoder schedule vs oracle: rel-L2", r, "cos", cs, "launches", emu_ops.digest(calls))
     assert r <= 3e-2 and cs >= 0.999, (r, cs)
+    assert emu_ops.digest(calls) == LAUNCHES["decoder_t3_deterministic"]
 
 
 # ---------------------------------------------------------------------------------------------------------------

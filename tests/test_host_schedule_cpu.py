@@ -34,13 +34,19 @@ DEC_KW = dict(attn_type="vanilla", double_z=True, z_channels=4, resolution=256, 
 
 # (ops calls, sha256 of the call sequence: entry point, tensor shapes / dtypes / strides, scalar arguments) of the
 # schedules below, recorded when the CPU suite still reached them through test-only subclasses and private `_run`
-# calls: reached through forward() / sample_views they must launch exactly the same kernels with the same arguments
+# calls: reached through forward() / sample_views they must launch exactly the same kernels with the same arguments.
+# The frame-sharded UNet ranks and the deterministic-mode schedules were recorded before the time_stack, ResnetBlock
+# and AttnBlock launches moved into shared helpers of KernelModule / FirstStage
 LAUNCHES = {
     "decoder_t3": (191, "fe7e4dfc0dc41f632bc332fbde1e75648f008d1065bf40de9b4eccfd837c2500"),
     "decoder_t5_rank0_of_2": (191, "b94005a5eda61ebe3d9eb9821a5050dbeaa51585ca109cbfc03002d119c06daf"),
     "decoder_t5_rank1_of_2": (191, "362197510c94f182a28cc70c75f786bb7031eef8b2e514aba5910207a48a2988"),
     "encoder_64": (83, "53e76c186384f95d11aa98266b7ee34267fdf66d34dc8d76fd58391277a8703b"),
     "sample_views": (1639, "a705de874c93f680b818978057b2369e95b6a8faf19e3f13591e145a948a8300"),
+    "unet_t5_rank0_of_2": (804, "534ce2260dbd140f9aa649c3f690d34b220f07eddf2bb8bb912b922bd73ce97b"),
+    "unet_t5_rank1_of_2": (804, "ac58c24c2b31b690605c6f24babb1a1662f342e905c58ccac7e063d32aea7697"),
+    "unet_t3_deterministic": (744, "63934c3e40e2a3a6eac4f8c5063471a720495992fe302626fca083a5c4023284"),
+    "decoder_t3_deterministic": (191, "6c5145ab17ad9dd9a2155d483e1436f0b0bfe8b6e3509f0c54e4083ad8e8e1a6"),
 }
 
 
@@ -149,7 +155,7 @@ def _shard_worker(rank: int, world: int, port: int, T: int, q):
     vs = ViewShard.create(T)
     res = {"rank": rank, "block": (vs.t0, vs.tl)}
     pick = torch.cat([torch.arange(vs.t0, vs.t0 + vs.tl), T + torch.arange(vs.t0, vs.t0 + vs.tl)])
-    calls = []
+    calls, ucalls = [], []
     with emu_ops.patched():
         net, _ = _build_unet()
         xin, ts, ctx, y = _unet_inputs(T, 16)
@@ -157,10 +163,12 @@ def _shard_worker(rank: int, world: int, port: int, T: int, q):
         tc = torch.stack([ctx[0], ctx[T]])                               # frame 0 of the uc and the c video
         net.view_shard = vs
         try:
-            part = net(xin[pick], ts[pick], ctx[pick], y[pick], time_context=tc, num_video_frames=vs.tl,
-                       image_only_indicator=torch.zeros(2, vs.tl))
+            with emu_ops.patched(ucalls):
+                part = net(xin[pick], ts[pick], ctx[pick], y[pick], time_context=tc, num_video_frames=vs.tl,
+                           image_only_indicator=torch.zeros(2, vs.tl))
         finally:
             net.view_shard = None
+        res["unet_launches"] = emu_ops.digest(ucalls)
         res["unet_rel"] = _rel(part, full[pick])
         res["unet_exchanges"] = dict(vs.exchanges)
 
@@ -192,6 +200,7 @@ def test_view_sharded_host_schedule_matches_unsharded_gloo():
         assert r["unet_rel"] <= 1e-6, r
         assert r["dec_rel"] <= 1e-6 and r["dec_gathered_rel"] <= 1e-6, r
         assert r["dec_launches"] == LAUNCHES[f"decoder_t5_rank{r['rank']}_of_2"], r
+        assert r["unet_launches"] == LAUNCHES[f"unet_t5_rank{r['rank']}_of_2"], r
         # UNet: 22 VideoResBlocks x (2 statistics all-reduces + 2 halo exchanges), 16 transformers x 1 K|V gather
         assert r["unet_exchanges"] == {"gn_allreduce": 44, "halo": 44, "kv_allgather": 16}, r
 

@@ -32,7 +32,7 @@ import torch.nn.functional as F
 
 from . import ops
 from .sampling import instantiate_from_config
-from .unet import KernelModule
+from .kernel_module import KernelModule
 
 CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)
 CLIP_STD = (0.26862954, 0.26130258, 0.27577711)

@@ -16,10 +16,11 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .unet import KernelModule, _register
+from .first_stage import FirstStage
+from .kernel_module import _register
 
 
-class VideoDecoder(KernelModule):
+class VideoDecoder(FirstStage):
     available_time_modes = ["all", "conv-only", "attn-only"]
 
     def __init__(
@@ -97,59 +98,36 @@ class VideoDecoder(KernelModule):
 
     def param_shapes(self) -> Dict[str, Tuple[int, ...]]:
         table: Dict[str, Tuple[int, ...]] = {}
-
-        def conv(key, co, ci, *ks):
-            table[key + ".weight"] = (co, ci, *ks)
-            table[key + ".bias"] = (co,)
-
-        def affine(key, c):
-            table[key + ".weight"] = (c,)
-            table[key + ".bias"] = (c,)
-
+        conv, affine = self._conv_shape, self._affine_shape
         top = self.ch * self.ch_mult[-1]
-        conv("conv_in", top, self.z_channels, 3, 3)
+        conv(table, "conv_in", top, self.z_channels, 3, 3)
         last = top
         for name, ci, co in self._blocks():
             if name.startswith("@attn:"):
-                key = name[6:]
-                affine(key + ".norm", ci)
-                for n in ("q", "k", "v", "proj_out"):
-                    conv(f"{key}.{n}", ci, ci, 1, 1)
+                self._attn_block_shapes(table, name[6:], ci)
             elif name.startswith("@up:"):
-                conv(name[4:], co, ci, 3, 3)
+                conv(table, name[4:], co, ci, 3, 3)
             else:
-                affine(name + ".norm1", ci)
-                conv(name + ".conv1", co, ci, 3, 3)
-                affine(name + ".norm2", co)
-                conv(name + ".conv2", co, co, 3, 3)
-                if ci != co:
-                    conv(name + ".nin_shortcut", co, ci, 1, 1)
+                self._resnet_block_shapes(table, name, ci, co)
                 ts = name + ".time_stack"
-                affine(ts + ".in_layers.0", co)
-                conv(ts + ".in_layers.2", co, co, 3, 1, 1)
-                affine(ts + ".out_layers.0", co)
-                conv(ts + ".out_layers.3", co, co, 3, 1, 1)
+                affine(table, ts + ".in_layers.0", co)
+                conv(table, ts + ".in_layers.2", co, co, 3, 1, 1)
+                affine(table, ts + ".out_layers.0", co)
+                conv(table, ts + ".out_layers.3", co, co, 3, 1, 1)
                 table[name + ".mix_factor"] = (1,)
             last = co
-        affine("norm_out", last)
-        conv("conv_out", self.out_ch, last, 3, 3)
-        conv("conv_out.time_mix_conv", self.out_ch, self.out_ch, 3, 1, 1)
+        affine(table, "norm_out", last)
+        conv(table, "conv_out", self.out_ch, last, 3, 3)
+        conv(table, "conv_out.time_mix_conv", self.out_ch, self.out_ch, 3, 1, 1)
         return table
 
     def _init_value(self, key: str, shape) -> torch.Tensor:
-        if torch.empty(0).device.type == "meta":
-            return torch.empty(shape)
-        if key.endswith("mix_factor"):
-            return torch.full(shape, float(self.alpha0))
-        if len(shape) == 1:
-            is_norm = "norm" in key.rsplit(".", 2)[-2] or ".in_layers.0." in key or ".out_layers.0." in key
-            if is_norm:
-                return torch.ones(shape) if key.endswith(".weight") else torch.zeros(shape)
-            return torch.zeros(shape)
-        if ".time_stack.out_layers.3." in key:
-            return torch.zeros(shape)  # zero_module (openaimodel.py:306-314)
-        bound = 1.0 / math.sqrt(math.prod(shape[1:]))
-        return (torch.rand(shape) * 2.0 - 1.0) * bound
+        if torch.empty(0).device.type != "meta":
+            if key.endswith("mix_factor"):
+                return torch.full(shape, float(self.alpha0))
+            if ".time_stack.out_layers.3." in key:
+                return torch.zeros(shape)  # zero_module (openaimodel.py:306-314)
+        return super()._init_value(key, shape)
 
     @torch.no_grad()
     def randomize_zero_modules_(self, seed: int = 1) -> "VideoDecoder":
@@ -169,16 +147,6 @@ class VideoDecoder(KernelModule):
     def _pack(self, dev: torch.device) -> dict:
         sd = {k: v.detach() for k, v in self.named_parameters()}
         P: dict = {}
-
-        def affine(key):
-            P[key + ".weight"] = self._f32(sd[key + ".weight"])
-            P[key + ".bias"] = self._f32(sd[key + ".bias"])
-
-        def conv1x1(key):
-            w = sd[key + ".weight"]
-            P[key + ".weight"] = self._bf(w.reshape(w.shape[0], w.shape[1]))
-            P[key + ".bias"] = self._f32(sd[key + ".bias"])
-
         kpad = (9 * self.z_channels + 63) // 64 * 64
         P["conv_in.weight"], P["conv_in.bias"] = self._pack_conv3x3(sd["conv_in.weight"], sd["conv_in.bias"], kpad)
         mix_keys = [k for k in sd if k.endswith("mix_factor")]
@@ -188,32 +156,14 @@ class VideoDecoder(KernelModule):
             P[k[:-len(".mix_factor")] + ".alpha"] = v if self.merge_strategy == "fixed" else 1.0 / (1.0 + math.exp(-v))
         for name, ci, co in self._blocks():
             if name.startswith("@attn:"):
-                key = name[6:]
-                affine(key + ".norm")
-                wq, wk = sd[key + ".q.weight"].reshape(ci, ci), sd[key + ".k.weight"].reshape(ci, ci)
-                P[key + ".qk.weight"] = self._bf(torch.cat([wq, wk], 0))
-                P[key + ".qk.bias"] = self._f32(torch.cat([sd[key + ".q.bias"], sd[key + ".k.bias"]], 0))
-                P[key + ".v.weight"] = self._bf(sd[key + ".v.weight"].reshape(ci, ci))
-                P[key + ".v.bias"] = self._f32(sd[key + ".v.bias"])
-                conv1x1(key + ".proj_out")
+                self._pack_attn_block(P, sd, name[6:], ci)
             elif name.startswith("@up:"):
                 key = name[4:]
                 P[key + ".weight"], P[key + ".bias"] = self._pack_conv3x3(sd[key + ".weight"], sd[key + ".bias"])
             else:
-                affine(name + ".norm1")
-                affine(name + ".norm2")
-                for cname in (".conv1", ".conv2"):
-                    P[name + cname + ".weight"], P[name + cname + ".bias"] = self._pack_conv3x3(
-                        sd[name + cname + ".weight"], sd[name + cname + ".bias"])
-                if ci != co:
-                    conv1x1(name + ".nin_shortcut")
-                ts = name + ".time_stack"
-                affine(ts + ".in_layers.0")
-                affine(ts + ".out_layers.0")
-                for cname in (".in_layers.2", ".out_layers.3"):
-                    P[ts + cname + ".weight"], P[ts + cname + ".bias"] = self._pack_tconv(
-                        sd[ts + cname + ".weight"], sd[ts + cname + ".bias"])
-        affine("norm_out")
+                self._pack_resnet_block(P, sd, name, ci, co)
+                self._pack_time_stack(P, sd, name + ".time_stack")
+        self._pack_affine(P, sd, "norm_out")
         P["conv_out.weight"], P["conv_out.bias"] = self._pack_conv3x3(sd["conv_out.weight"], sd["conv_out.bias"])
         P["time_mix.weight"] = self._f32(sd["conv_out.time_mix_conv.weight"].reshape(self.out_ch, self.out_ch, 3))
         P["time_mix.bias"] = self._f32(sd["conv_out.time_mix_conv.bias"])
@@ -223,55 +173,8 @@ class VideoDecoder(KernelModule):
     def _video_res_block(self, P, name, ci, co, x, B, T, nb, h, w):
         """temporal_ae.VideoResBlock.forward (temporal_ae.py:64-83): ResnetBlock (model.py:131-151), then
         alpha * time_stack(x) + (1 - alpha) * x  ==  x + alpha * conv_t(...)."""
-        hw = h * w
-        rows = B * hw
-        a = self._gn(P, name + ".norm1", x, hw, B, ci, 1e-6, True)
-        h1 = self._conv3x3(P, name + ".conv1", a, B, h, w, ci)
-        a = self._gn(P, name + ".norm2", h1, hw, B, co, 1e-6, True)
-        skip = x if ci == co else self._linear(P, name + ".nin_shortcut", x, rows)
-        xs = self._conv3x3(P, name + ".conv2", a, B, h, w, co, r1=skip, s1=1.0, out=h1)
-        # (frame-sharded: T is this rank's block; the 3-D norms all-reduce their statistics, the convs read halos)
-        ts = name + ".time_stack"
-        norm = self._gn_halo if self.view_shard is not None else None
-        a = (norm(P, ts + ".in_layers.0", xs, hw, T, nb, co, 1e-5, True) if norm else
-             self._gn(P, ts + ".in_layers.0", xs, T * hw, nb, co, 1e-5, True, hw=hw))
-        h2 = torch.empty(rows, co, device=x.device, dtype=torch.bfloat16)
-        self._tconv(P, ts + ".in_layers.2", a, h2, hw, T, nb, co)
-        a = (norm(P, ts + ".out_layers.0", h2, hw, T, nb, co, 1e-5, True) if norm else
-             self._gn(P, ts + ".out_layers.0", h2, T * hw, nb, co, 1e-5, True, hw=hw))
-        self._tconv(P, ts + ".out_layers.3", a, h2, hw, T, nb, co, r1=xs, s1=1.0, s0=P[name + ".alpha"])
-        return h2
-
-    def _attn(self, P, key, c, x, B, h, w):
-        """AttnBlock (model.py:161-201): single head, d = C, over h*w tokens per frame.
-        S = q k^T (fp32), softmax, O = P v; v's bias is added after P.v (rows of P sum to 1)."""
-        hw = h * w
-        rows = B * hw
-        dev = x.device
-        xn = self._gn(P, key + ".norm", x, hw, B, c, 1e-6, False)
-        qk = self._linear(P, key + ".qk", xn, rows)                       # [rows, 2C]: q | k
-        # V^T for all frames: vt[d, f*hw + j] = sum_k Wv[d,k] xn[f*hw + j, k]
-        vt = torch.empty(c, rows, device=dev, dtype=torch.bfloat16)
-        ops.gemm(P[key + ".v.weight"], xn, vt, K=c, N=rows, rows_per_batch=c)
-        scores = torch.empty(B, hw, hw, device=dev, dtype=torch.float32)
-        k_view = qk[:, c:]
-        ops.gemm(qk, k_view, scores, K=c, N=hw, rows_per_batch=hw, batch=B, lda=2 * c, ldb=2 * c,
-                 a_batch_stride=hw * 2 * c, b_batch_stride=hw * 2 * c)
-        probs = torch.empty(B, hw, hw, device=dev, dtype=torch.bfloat16)
-        ops.softmax_rows_f32(scores, probs, B * hw, hw, float(c) ** -0.5)
-        del scores
-        o = torch.empty(rows, c, device=dev, dtype=torch.bfloat16)
-        ops.gemm(probs, vt, o, K=hw, N=c, rows_per_batch=hw, batch=B, a_batch_stride=hw * hw, ldb=rows,
-                 b_batch_stride=hw, bias=P[key + ".v.bias"])
-        return self._linear(P, key + ".proj_out", o, rows, out=xn, r1=x, s1=1.0)
-
-    def _tap(self, name, x, B, c, h, w):
-        """With `debug_taps` holding `name`: the block output x (bf16 NHWC) widened to fp32 NCHW, which is exactly
-        the next block's input.  Launches nothing when taps are off."""
-        if self.debug_taps is not None and name in self.debug_taps:
-            tap = torch.empty(B, c, h, w, device=x.device, dtype=torch.float32)
-            ops.nhwc_to_nchw_f32(x, tap, B, c, h * w, c)
-            self.debug_taps[name] = tap
+        xs = self._resnet_block(P, name, ci, co, x, B, h, w)
+        return self._time_stack(P, name + ".time_stack", xs, h * w, T, nb, co, s0=P[name + ".alpha"])
 
     def forward(self, z: torch.Tensor, timesteps: Optional[int] = None, skip_video: bool = False, **kwargs):
         if skip_video:
@@ -298,8 +201,7 @@ class VideoDecoder(KernelModule):
             vs.begin("decoder")
         dev, zc = z.device, self.z_channels
         n_norms = 4 * sum(1 for n, _, _ in self._blocks() if not n.startswith("@")) + 2
-        object.__setattr__(self, "_gn_pool", [torch.zeros(n_norms * B * 64, device=dev, dtype=torch.float64), 0])
-        try:
+        with self._stats_pool(n_norms * B, dev):
             cur = torch.empty(B * H * W, zc, device=dev, dtype=torch.bfloat16)
             ops.nchw_f32_to_nhwc_bf16(z.float().contiguous(), cur)
             h, w = H, W
@@ -338,8 +240,6 @@ class VideoDecoder(KernelModule):
                 ops.time_mix_conv(pad.view(-1, cop), cop, P["time_mix.weight"], P["time_mix.bias"], full, 1, T + 2,
                                   h * w, self.out_ch)
                 out = full[1:T + 1].contiguous()
-        finally:
-            object.__setattr__(self, "_gn_pool", None)   # also after a failed run (OOM mid-schedule)
         return out
 
 

@@ -13,17 +13,16 @@ checked against them in tests/test_parity_gpu.py::test_encoder_matches_reference
 """
 from __future__ import annotations
 
-import math
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 
 from . import ops
-from .decoder import VideoDecoder
-from .unet import KernelModule, _register
+from .first_stage import FirstStage
+from .kernel_module import _register
 
 
-class Encoder(KernelModule):
+class Encoder(FirstStage):
     def __init__(
         self,
         *,
@@ -85,101 +84,40 @@ class Encoder(KernelModule):
 
     def param_shapes(self) -> Dict[str, Tuple[int, ...]]:
         table: Dict[str, Tuple[int, ...]] = {}
-
-        def conv(key, co, ci, k):
-            table[key + ".weight"] = (co, ci, k, k)
-            table[key + ".bias"] = (co,)
-
-        def affine(key, c):
-            table[key + ".weight"] = (c,)
-            table[key + ".bias"] = (c,)
-
-        conv("conv_in", self.ch, self.in_channels, 3)
+        conv = self._conv_shape
+        conv(table, "conv_in", self.ch, self.in_channels, 3, 3)
         last = self.ch
         for name, ci, co in self._blocks():
             if name.startswith("@attn:"):
-                key = name[6:]
-                affine(key + ".norm", ci)
-                for n in ("q", "k", "v", "proj_out"):
-                    conv(f"{key}.{n}", ci, ci, 1)
+                self._attn_block_shapes(table, name[6:], ci)
             elif name.startswith("@down:"):
-                conv(name[6:], co, ci, 3)
+                conv(table, name[6:], co, ci, 3, 3)
             else:
-                affine(name + ".norm1", ci)
-                conv(name + ".conv1", co, ci, 3)
-                affine(name + ".norm2", co)
-                conv(name + ".conv2", co, co, 3)
-                if ci != co:
-                    conv(name + ".nin_shortcut", co, ci, 1)
+                self._resnet_block_shapes(table, name, ci, co)
             last = co
-        affine("norm_out", last)
-        conv("conv_out", self.out_channels, last, 3)
+        self._affine_shape(table, "norm_out", last)
+        conv(table, "conv_out", self.out_channels, last, 3, 3)
         return table
-
-    def _init_value(self, key: str, shape) -> torch.Tensor:
-        if torch.empty(0).device.type == "meta":
-            return torch.empty(shape)
-        if len(shape) == 1:
-            if "norm" in key.rsplit(".", 2)[-2]:
-                return torch.ones(shape) if key.endswith(".weight") else torch.zeros(shape)
-            return torch.zeros(shape)
-        bound = 1.0 / math.sqrt(math.prod(shape[1:]))
-        return (torch.rand(shape) * 2.0 - 1.0) * bound
 
     # --------------------------------------------------------------------------------------------
     def _pack(self, dev: torch.device) -> dict:
         sd = {k: v.detach() for k, v in self.named_parameters()}
         P: dict = {}
-
-        def affine(key):
-            P[key + ".weight"] = self._f32(sd[key + ".weight"])
-            P[key + ".bias"] = self._f32(sd[key + ".bias"])
-
-        def conv1x1(key):
-            w = sd[key + ".weight"]
-            P[key + ".weight"] = self._bf(w.reshape(w.shape[0], w.shape[1]))
-            P[key + ".bias"] = self._f32(sd[key + ".bias"])
-
         kpad = (9 * self.in_channels + 63) // 64 * 64
         P["conv_in.weight"], P["conv_in.bias"] = self._pack_conv3x3(sd["conv_in.weight"], sd["conv_in.bias"], kpad)
         for name, ci, co in self._blocks():
             if name.startswith("@attn:"):
-                key = name[6:]
-                affine(key + ".norm")
-                wq, wk = sd[key + ".q.weight"].reshape(ci, ci), sd[key + ".k.weight"].reshape(ci, ci)
-                P[key + ".qk.weight"] = self._bf(torch.cat([wq, wk], 0))
-                P[key + ".qk.bias"] = self._f32(torch.cat([sd[key + ".q.bias"], sd[key + ".k.bias"]], 0))
-                P[key + ".v.weight"] = self._bf(sd[key + ".v.weight"].reshape(ci, ci))
-                P[key + ".v.bias"] = self._f32(sd[key + ".v.bias"])
-                conv1x1(key + ".proj_out")
+                self._pack_attn_block(P, sd, name[6:], ci)
             elif name.startswith("@down:"):
                 key = name[6:]
                 P[key + ".weight"], P[key + ".bias"] = self._pack_conv3x3(sd[key + ".weight"], sd[key + ".bias"])
             else:
-                affine(name + ".norm1")
-                affine(name + ".norm2")
-                for cname in (".conv1", ".conv2"):
-                    P[name + cname + ".weight"], P[name + cname + ".bias"] = self._pack_conv3x3(
-                        sd[name + cname + ".weight"], sd[name + cname + ".bias"])
-                if ci != co:
-                    conv1x1(name + ".nin_shortcut")
-        affine("norm_out")
+                self._pack_resnet_block(P, sd, name, ci, co)
+        self._pack_affine(P, sd, "norm_out")
         P["conv_out.weight"], P["conv_out.bias"] = self._pack_conv3x3(sd["conv_out.weight"], sd["conv_out.bias"])
         return P
 
     # --------------------------------------------------------------------------------------------
-    _attn = VideoDecoder._attn  # AttnBlock (model.py:161-201): same single-head block as the decoder's mid.attn_1
-    _tap = VideoDecoder._tap
-
-    def _res_block(self, P, name, ci, co, x, B, h, w):
-        """ResnetBlock.forward with temb = None (model.py:131-151)."""
-        hw = h * w
-        a = self._gn(P, name + ".norm1", x, hw, B, ci, 1e-6, True)
-        h1 = self._conv3x3(P, name + ".conv1", a, B, h, w, ci)
-        a = self._gn(P, name + ".norm2", h1, hw, B, co, 1e-6, True)
-        skip = x if ci == co else self._linear(P, name + ".nin_shortcut", x, B * hw)
-        return self._conv3x3(P, name + ".conv2", a, B, h, w, co, r1=skip, s1=1.0, out=h1)
-
     def _downsample(self, P, key, x, B, h, w, c):
         """Downsample (model.py:74-91): F.pad (0,1,0,1) then Conv2d(k=3, stride=2, padding=0): the zero padding is
         bottom/right only, so the im2row runs with pad 0 and output size h/2 x w/2."""
@@ -205,8 +143,7 @@ class Encoder(KernelModule):
         B, cin, H, W = x.shape
         dev = x.device
         n_norms = 2 * sum(1 for n, _, _ in self._blocks() if not n.startswith("@")) + 2
-        object.__setattr__(self, "_gn_pool", [torch.zeros(n_norms * B * 64, device=dev, dtype=torch.float64), 0])
-        try:
+        with self._stats_pool(n_norms * B, dev):
             cur = torch.empty(B * H * W, cin, device=dev, dtype=torch.bfloat16)
             ops.nchw_f32_to_nhwc_bf16(x.float().contiguous(), cur)
             h, w = H, W
@@ -221,15 +158,13 @@ class Encoder(KernelModule):
                 elif name.startswith("@down:"):
                     cur, h, w = self._downsample(P, name[6:], cur, B, h, w, ci)
                 else:
-                    cur = self._res_block(P, name, ci, co, cur, B, h, w)
+                    cur = self._resnet_block(P, name, ci, co, cur, B, h, w)
                     ch = co
                 self._tap(name.rsplit(":", 1)[-1], cur, B, ch, h, w)
             a = self._gn(P, "norm_out", cur, h * w, B, ch, 1e-6, True)
             o = self._conv3x3(P, "conv_out", a, B, h, w, ch, out_dtype=torch.float32)   # [rows, 16] fp32
             out = torch.empty(B, self.out_channels, h, w, device=dev, dtype=torch.float32)
             ops.nhwc_to_nchw_f32(o, out, B, self.out_channels, h * w, ldx=o.shape[1])
-        finally:
-            object.__setattr__(self, "_gn_pool", None)   # also after a failed run (OOM mid-schedule)
         return out
 
 

@@ -16,6 +16,7 @@
 namespace v3d {
 
 constexpr int HD = 64;  // head dim
+constexpr float kLog2e = 1.44269504088896340736f;
 
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem, bool valid) {
   const int sz = valid ? 16 : 0;
@@ -253,18 +254,20 @@ constexpr int kTaTile = 32 * 128;  // one [32 rows][64] bf16 tile, 128-byte rows
 //
 // SPLIT (frame-sharded views, SURVEY 8(e)): the T query frames are this rank's block of the video while keys and
 // values come from all kv.tk frames of the K|V all-gather buffer, whose rows are rank-major: row of key frame f,
-// CFG half b, pixel s is kv.row[f] + b * kv.bstride[f] + s (row stride ldkv).  Keys >= kv.tk are masked.
-struct TaKV {
+// CFG half b, pixel s is kv.row[f] + b * kv.bstride[f] + s (row stride ldkv).  Keys >= kv.tk are masked.  The dense
+// form has kv.tk = T and leaves the table zero.  N = 32 here, 128 for attn_temporal_long_kernel.
+template <int N>
+struct KvRows {
   int tk;
-  int row[kMaxT];
-  int bstride[kMaxT];
+  int row[N];
+  int bstride[N];
 };
 
 template <bool SPLIT>
 __global__ void __launch_bounds__(kTaWarps * 32)
 attn_temporal_kernel(const bf16* __restrict__ Q, const bf16* __restrict__ K, const bf16* __restrict__ V,
                      bf16* __restrict__ O, long long ld, long long ldo, int T, int S, int nheads,
-                     float scale_log2e, long long ldkv, const __grid_constant__ TaKV kv) {
+                     float scale_log2e, long long ldkv, const __grid_constant__ KvRows<kMaxT> kv) {
   extern __shared__ __align__(128) uint8_t ta_smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
@@ -447,7 +450,7 @@ attn_temporal_kernel(const bf16* __restrict__ Q, const bf16* __restrict__ K, con
 // four warp-private sequences would take 192 KB and leave one CTA of 4 warps per SM, far too few loads in flight for
 // a kernel that is bound by its HBM gathers.  Here the CTA's 4 warps share one K and one V tile and split the 16-query
 // m-tiles between them (warp w takes m-tiles w, w + 4): 48 KB at T = 128, 18 KB at T = 48, all within the 48 KB that
-// need no opt-in.  ptxas: 110 registers (KT = 8) and 82 (KT = 4), no spills, so 4 CTAs of 128 threads fit an SM by
+// need no opt-in.  ptxas: 108 / 110 registers (KT = 8) and 82 / 78 (KT = 4), no spills, so 4 CTAs of 128 threads fit an SM by
 // registers and by shared memory even at T = 128 (4 x 48 KB), each with its whole gather in flight before its first
 // MMA; the launch bounds only keep the compiler from growing past 3 (KT = 8) / 4 (KT = 4) resident CTAs' worth.
 //
@@ -464,17 +467,11 @@ attn_temporal_kernel(const bf16* __restrict__ Q, const bf16* __restrict__ K, con
 constexpr int kMaxTLong = 128;
 constexpr int kTlWarps = 4;
 
-struct TaKVLong {
-  int tk;
-  int row[kMaxTLong];
-  int bstride[kMaxTLong];
-};
-
 template <bool SPLIT, int KT>
 __global__ void __launch_bounds__(kTlWarps * 32, KT == 4 ? 4 : 3)
 attn_temporal_long_kernel(const bf16* __restrict__ Q, const bf16* __restrict__ K, const bf16* __restrict__ V,
                           bf16* __restrict__ O, long long ld, long long ldo, int T, int S, float scale_log2e,
-                          long long ldkv, const __grid_constant__ TaKVLong kv) {
+                          long long ldkv, const __grid_constant__ KvRows<kMaxTLong> kv) {
   extern __shared__ __align__(128) uint8_t tl_smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
@@ -604,22 +601,69 @@ attn_temporal_long_kernel(const bf16* __restrict__ Q, const bf16* __restrict__ K
   }
 }
 
-// Host side of both temporal entry points for 32 < Tk <= 128.
+// Row table of the frame-sharded form from the host arrays kv_row / kv_bstride.  The dense form passes null and gets a
+// zero table, so a negative offset (the error names the _kv entry point) can only come from v3d_attention_temporal_kv.
+template <int N>
+static bool fill_kv_rows(KvRows<N>& kv, int Tk, const int32_t* kv_row, const int32_t* kv_bstride) {
+  memset(&kv, 0, sizeof(kv));
+  kv.tk = Tk;
+  for (int f = 0; kv_row && f < Tk; ++f) {
+    if (kv_row[f] < 0 || kv_bstride[f] < 0) {
+      set_error("v3d_attention_temporal_kv: negative row offset for key frame %d", f);
+      return false;
+    }
+    kv.row[f] = kv_row[f];
+    kv.bstride[f] = kv_bstride[f];
+  }
+  return true;
+}
+
+// Host side of both temporal entry points: attn_temporal_kernel for Tk <= 32 key frames, attn_temporal_long_kernel
+// (KT = 4 up to 64 key frames, 8 above) for 32 < Tk <= 128.
 template <bool SPLIT>
-static void launch_temporal_long(const void* q, const void* k, const void* v, void* o, int64_t ld_q, int64_t ld_kv,
-                                 int64_t ld_o, int nb, int Tq, int S, int nheads, float scale, const TaKVLong& kv,
-                                 cudaStream_t st) {
-  const int smem = (((Tq + 15) & ~15) + 2 * ((kv.tk + 15) & ~15)) * 128;   // <= 48 KB: no opt-in needed
-  dim3 grid(S, nheads, nb);
-  const float sl2 = scale * 1.44269504088896340736f;
-  if (kv.tk <= 64)
-    attn_temporal_long_kernel<SPLIT, 4><<<grid, kTlWarps * 32, smem, st>>>(
-        static_cast<const bf16*>(q), static_cast<const bf16*>(k), static_cast<const bf16*>(v),
-        static_cast<bf16*>(o), ld_q, ld_o, Tq, S, sl2, ld_kv, kv);
+static int launch_temporal(const void* q, const void* k, const void* v, void* o, int64_t ld_q, int64_t ld_kv,
+                           int64_t ld_o, int nb, int Tq, int Tk, int S, int nheads, float scale,
+                           const int32_t* kv_row, const int32_t* kv_bstride, cudaStream_t st) {
+  const bf16 *Q = static_cast<const bf16*>(q), *K = static_cast<const bf16*>(k), *V = static_cast<const bf16*>(v);
+  bf16* O = static_cast<bf16*>(o);
+  const float sl2 = scale * kLog2e;
+  if (Tk <= kMaxT) {
+    KvRows<kMaxT> kv;
+    if (!fill_kv_rows(kv, Tk, kv_row, kv_bstride)) return V3D_ERR_BAD_ARG;
+    attn_temporal_kernel<SPLIT><<<dim3(S, nb), kTaWarps * 32, kTaWarps * 3 * kTaTile, st>>>(
+        Q, K, V, O, ld_q, ld_o, Tq, S, nheads, sl2, ld_kv, kv);
+    V3D_CHECK_LAUNCH(SPLIT ? "attn_temporal_kernel<split>" : "attn_temporal_kernel");
+    return V3D_OK;
+  }
+  KvRows<kMaxTLong> kv;
+  if (!fill_kv_rows(kv, Tk, kv_row, kv_bstride)) return V3D_ERR_BAD_ARG;
+  const int smem = (((Tq + 15) & ~15) + 2 * ((Tk + 15) & ~15)) * 128;  // <= 48 KB: no opt-in needed
+  const dim3 grid(S, nheads, nb);
+  if (Tk <= 64)
+    attn_temporal_long_kernel<SPLIT, 4><<<grid, kTlWarps * 32, smem, st>>>(Q, K, V, O, ld_q, ld_o, Tq, S, sl2, ld_kv,
+                                                                           kv);
   else
-    attn_temporal_long_kernel<SPLIT, 8><<<grid, kTlWarps * 32, smem, st>>>(
-        static_cast<const bf16*>(q), static_cast<const bf16*>(k), static_cast<const bf16*>(v),
-        static_cast<bf16*>(o), ld_q, ld_o, Tq, S, sl2, ld_kv, kv);
+    attn_temporal_long_kernel<SPLIT, 8><<<grid, kTlWarps * 32, smem, st>>>(Q, K, V, O, ld_q, ld_o, Tq, S, sl2, ld_kv,
+                                                                           kv);
+  V3D_CHECK_LAUNCH(SPLIT ? "attn_temporal_long_kernel<split>" : "attn_temporal_long_kernel");
+  return V3D_OK;
+}
+
+// Host side of the spatial twin: 128-query CTAs (48 KB of shared memory, opted in) from 512 tokens up, 64 below.
+template <int BM>
+static void launch_spatial(const void* q, const void* k, const void* v, void* o, int64_t ld_qkv, int64_t ld_o,
+                           int nbatch, int ntok, int nheads, float scale, cudaStream_t st) {
+  const int smem = BM * 128 + 4 * FA_BN * 128;
+  if constexpr (BM == 128) {
+    static bool cfg = false;
+    if (!cfg) {
+      cudaFuncSetAttribute(attn_spatial_kernel<BM>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+      cfg = true;
+    }
+  }
+  attn_spatial_kernel<BM><<<dim3((ntok + BM - 1) / BM, nheads, nbatch), BM * 2, smem, st>>>(
+      static_cast<const bf16*>(q), static_cast<const bf16*>(k), static_cast<const bf16*>(v), static_cast<bf16*>(o),
+      ld_qkv, ld_o, ntok, scale * kLog2e);
 }
 
 }  // namespace v3d
@@ -641,27 +685,10 @@ int v3d_attention_spatial_mma(const void* q, const void* k, const void* v, void*
     return V3D_ERR_BAD_ARG;
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const float sl2 = scale * 1.44269504088896340736f;
-  if (ntok >= 512) {
-    constexpr int BM = 128;
-    const int smem = BM * 128 + 4 * FA_BN * 128;
-    static bool cfg = false;
-    if (!cfg) {
-      cudaFuncSetAttribute(attn_spatial_kernel<BM>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-      cfg = true;
-    }
-    dim3 grid((ntok + BM - 1) / BM, nheads, nbatch);
-    attn_spatial_kernel<BM><<<grid, BM * 2, smem, st>>>(
-        static_cast<const bf16*>(q), static_cast<const bf16*>(k), static_cast<const bf16*>(v),
-        static_cast<bf16*>(o), ld_qkv, ld_o, ntok, sl2);
-  } else {
-    constexpr int BM = 64;
-    const int smem = BM * 128 + 4 * FA_BN * 128;
-    dim3 grid((ntok + BM - 1) / BM, nheads, nbatch);
-    attn_spatial_kernel<BM><<<grid, BM * 2, smem, st>>>(
-        static_cast<const bf16*>(q), static_cast<const bf16*>(k), static_cast<const bf16*>(v),
-        static_cast<bf16*>(o), ld_qkv, ld_o, ntok, sl2);
-  }
+  if (ntok >= 512)
+    launch_spatial<128>(q, k, v, o, ld_qkv, ld_o, nbatch, ntok, nheads, scale, st);
+  else
+    launch_spatial<64>(q, k, v, o, ld_qkv, ld_o, nbatch, ntok, nheads, scale, st);
   V3D_CHECK_LAUNCH("attn_spatial_kernel");
   return V3D_OK;
 }
@@ -676,25 +703,8 @@ int v3d_attention_temporal(const void* q, const void* k, const void* v, void* o,
               "key tiles, which this kernel family does not have)", T, kMaxTLong);
     return V3D_ERR_BAD_ARG;
   }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (T > kMaxT) {
-    TaKVLong none;
-    memset(&none, 0, sizeof(none));
-    none.tk = T;
-    launch_temporal_long<false>(q, k, v, o, ld_qkv, ld_qkv, ld_o, nb, T, S, nheads, scale, none, st);
-    V3D_CHECK_LAUNCH("attn_temporal_long_kernel");
-    return V3D_OK;
-  }
-  const int smem = kTaWarps * 3 * kTaTile;
-  dim3 grid(S, nb);
-  TaKV none;
-  memset(&none, 0, sizeof(none));
-  none.tk = T;
-  attn_temporal_kernel<false><<<grid, kTaWarps * 32, smem, st>>>(
-      static_cast<const bf16*>(q), static_cast<const bf16*>(k), static_cast<const bf16*>(v),
-      static_cast<bf16*>(o), ld_qkv, ld_o, T, S, nheads, scale * 1.44269504088896340736f, ld_qkv, none);
-  V3D_CHECK_LAUNCH("attn_temporal_kernel");
-  return V3D_OK;
+  return launch_temporal<false>(q, k, v, o, ld_qkv, ld_qkv, ld_o, nb, T, T, S, nheads, scale, nullptr, nullptr,
+                                static_cast<cudaStream_t>(stream));
 }
 
 /* Frame-sharded temporal self-attention (SURVEY.md 8(e); BASELINE.json "temporal-attention KV all-gather"): this
@@ -712,42 +722,8 @@ int v3d_attention_temporal_kv(const void* q, const void* k, const void* v, void*
               "online softmax over key tiles, which this kernel family does not have)", Tq, Tk, kMaxTLong);
     return V3D_ERR_BAD_ARG;
   }
-  if (Tk > kMaxT) {
-    TaKVLong kvl;
-    memset(&kvl, 0, sizeof(kvl));
-    kvl.tk = Tk;
-    for (int f = 0; f < Tk; ++f) {
-      if (kv_row[f] < 0 || kv_bstride[f] < 0) {
-        set_error("v3d_attention_temporal_kv: negative row offset for key frame %d", f);
-        return V3D_ERR_BAD_ARG;
-      }
-      kvl.row[f] = kv_row[f];
-      kvl.bstride[f] = kv_bstride[f];
-    }
-    launch_temporal_long<true>(q, k, v, o, ld_q, ld_kv, ld_o, nb, Tq, S, nheads, scale, kvl,
+  return launch_temporal<true>(q, k, v, o, ld_q, ld_kv, ld_o, nb, Tq, Tk, S, nheads, scale, kv_row, kv_bstride,
                                static_cast<cudaStream_t>(stream));
-    V3D_CHECK_LAUNCH("attn_temporal_long_kernel<split>");
-    return V3D_OK;
-  }
-  TaKV kv;
-  memset(&kv, 0, sizeof(kv));
-  kv.tk = Tk;
-  for (int f = 0; f < Tk; ++f) {
-    if (kv_row[f] < 0 || kv_bstride[f] < 0) {
-      set_error("v3d_attention_temporal_kv: negative row offset for key frame %d", f);
-      return V3D_ERR_BAD_ARG;
-    }
-    kv.row[f] = kv_row[f];
-    kv.bstride[f] = kv_bstride[f];
-  }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int smem = kTaWarps * 3 * kTaTile;
-  dim3 grid(S, nb);
-  attn_temporal_kernel<true><<<grid, kTaWarps * 32, smem, st>>>(
-      static_cast<const bf16*>(q), static_cast<const bf16*>(k), static_cast<const bf16*>(v),
-      static_cast<bf16*>(o), ld_q, ld_o, Tq, S, nheads, scale * 1.44269504088896340736f, ld_kv, kv);
-  V3D_CHECK_LAUNCH("attn_temporal_kernel<split>");
-  return V3D_OK;
 }
 
 }  // extern "C"
